@@ -16,25 +16,14 @@
 // Algorithmic HBM bytes per pixel (fp32): fwd 32 (d1 4, d2 4, flow 8, mask 4, sf 12);
 // bwd 48 (the same 32 read + g_sf 12 + g_d2 4 written). See DESIGN.md for the full accounting.
 #include "common.cuh"
+#include <algorithm>
+#include <initializer_list>
 #include <mutex>
 #include <utility>
 #include <vector>
 #include "tc_common.cuh"
-#include <initializer_list>
-#include <stdlib.h>
-#include <atomic>
 
 namespace dvd {
-
-struct __align__(16) Pose {
-  float Kinv[9], K[9], R1[9], R2[9], t1[3], t2[3];
-  // derived once per block (column-vector algebra, c = (x, y, 1)^T):
-  float M1[9];   // R1 * Kinv                 P1  = d1 * (M1 c) + t1
-  float A[9];    // R2^T * R1 * Kinv          p12 = d1 * (A c) + cv + R2^T sf
-  float cv[3];   // R2^T (t1 - t2)
-  float pad;
-};
-static_assert(sizeof(Pose) == 64 * sizeof(float), "pose layout");
 
 // MUFU.RCP: max relative error 2^-23 (1 ulp), no slow path; inputs here are >= 1e-3 or flagged invalid
 __device__ __forceinline__ float rcp_fast(float v) {
@@ -53,28 +42,16 @@ __device__ __forceinline__ void mm3(const float* X, const float* Y, float* Z, bo
     }
 }
 
-__device__ __forceinline__ void load_pose(Pose& dst, const float* __restrict__ poses, int b) {
-  // cooperative copy of one pair's pose block into shared memory + derived matrices
-  float* d = reinterpret_cast<float*>(&dst);
-  for (int i = threadIdx.x; i < 42; i += blockDim.x) d[i] = __ldg(poses + (size_t)b * DVD_POSE_STRIDE + i);
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    mm3(dst.R1, dst.Kinv, dst.M1, false);
-    mm3(dst.R2, dst.M1, dst.A, true);
-    float dx = dst.t1[0] - dst.t2[0], dy = dst.t1[1] - dst.t2[1], dz = dst.t1[2] - dst.t2[2];
-    for (int i = 0; i < 3; ++i) dst.cv[i] = fmaf(dst.R2[6 + i], dz, fmaf(dst.R2[3 + i], dy, dst.R2[i] * dx));
-  }
-}
-
+// M * v  /  M^T * v, every operation rounded on its own (no contraction the compiler could choose differently per kernel)
 __device__ __forceinline__ void mv(const float* M, float x, float y, float z, float& ox, float& oy, float& oz) {
-  ox = fmaf(M[2], z, fmaf(M[1], y, M[0] * x));
-  oy = fmaf(M[5], z, fmaf(M[4], y, M[3] * x));
-  oz = fmaf(M[8], z, fmaf(M[7], y, M[6] * x));
+  ox = fmaf(M[2], z, fmaf(M[1], y, __fmul_rn(M[0], x)));
+  oy = fmaf(M[5], z, fmaf(M[4], y, __fmul_rn(M[3], x)));
+  oz = fmaf(M[8], z, fmaf(M[7], y, __fmul_rn(M[6], x)));
 }
 __device__ __forceinline__ void mtv(const float* M, float x, float y, float z, float& ox, float& oy, float& oz) {
-  ox = fmaf(M[6], z, fmaf(M[3], y, M[0] * x));
-  oy = fmaf(M[7], z, fmaf(M[4], y, M[1] * x));
-  oz = fmaf(M[8], z, fmaf(M[5], y, M[2] * x));
+  ox = fmaf(M[6], z, fmaf(M[3], y, __fmul_rn(M[0], x)));
+  oy = fmaf(M[7], z, fmaf(M[4], y, __fmul_rn(M[1], x)));
+  oz = fmaf(M[8], z, fmaf(M[5], y, __fmul_rn(M[2], x)));
 }
 // M * (x, y, 1)
 __device__ __forceinline__ void ray_of(const float* M, float x, float y, float& rx, float& ry, float& rz) {
@@ -83,103 +60,8 @@ __device__ __forceinline__ void ray_of(const float* M, float x, float y, float& 
   rz = fmaf(M[7], y, M[6] * x) + M[8];
 }
 
-// Bilinear taps of ATen grid_sampler_2d(bilinear, padding_mode=border, align_corners=True) at the pixel
-// coordinate (qx,qy). The reference normalises to [-1,1] (losses/...:107-110) and ATen un-normalises
-// again; that round trip is the identity up to ~1e-7 relative (4e-5 px at W=384), far below the 1e-3
-// parity bar, so it is skipped (4 IEEE divisions per pixel).
-struct Taps {
-  int idx[4];    // linear index y*W+x of nw, ne, sw, se (clamped in range)
-  float w[4];    // weights, 0 for out-of-range taps
-  float ux[2], uy[2];  // tap coordinates as floats: x0,x1 / y0,y1
-};
-__device__ __forceinline__ Taps make_taps(float qx, float qy, int H, int W) {
-  const float hw = (float)(W - 1), hh = (float)(H - 1);
-  float ix = fminf(hw, fmaxf(qx, 0.0f));
-  float iy = fminf(hh, fmaxf(qy, 0.0f));
-  float x0f = floorf(ix), y0f = floorf(iy);
-  float wx1 = ix - x0f, wy1 = iy - y0f;
-  float wx0 = 1.0f - wx1, wy0 = 1.0f - wy1;
-  int x0 = (int)x0f, y0 = (int)y0f;
-  bool vx1 = x0 + 1 <= W - 1, vy1 = y0 + 1 <= H - 1;
-  int x1c = vx1 ? x0 + 1 : x0, y1c = vy1 ? y0 + 1 : y0;
-  Taps t;
-  t.idx[0] = y0 * W + x0;
-  t.idx[1] = y0 * W + x1c;
-  t.idx[2] = y1c * W + x0;
-  t.idx[3] = y1c * W + x1c;
-  t.w[0] = wx0 * wy0;
-  t.w[1] = vx1 ? wx1 * wy0 : 0.0f;
-  t.w[2] = vy1 ? wx0 * wy1 : 0.0f;
-  t.w[3] = (vx1 && vy1) ? wx1 * wy1 : 0.0f;
-  t.ux[0] = x0f; t.ux[1] = (float)x1c;
-  t.uy[0] = y0f; t.uy[1] = (float)y1c;
-  return t;
-}
-
-// Everything the forward chain produces for one pixel.
-struct Px {
-  float P1[3];      // global_p1
-  float wpc[3];     // warped_p2_camera_2
-  float wP2[3];     // warped_global_p2
-  float wd;         // depth_warp_1_2
-  float p12[3];     // p1_camera_2
-  float i12[3];     // K * p12 (z = depth_image_1_2)
-  float dflow[2];   // dflow_1_2
-  float rz;         // 1 / (i12.z + 1e-8)
-  bool zok;         // i12.z >= 1e-3 (projection used; otherwise own coordinate, zero gradient)
-};
-
-// kNeedWorld: also produce P1 and warped_global_p2 (only the sf_loss term / materialisation need them)
-template <bool kNeedWorld>
-__device__ __forceinline__ void forward_px(const Pose& ps, const float* __restrict__ d2img, const Taps& tp,
-                                           float x, float y, float d1, float sfx, float sfy, float sfz, Px& o) {
-  // bilinear gather: wpc = sum_k w_k d2_k Kinv (u_k, v_k, 1) = Kinv * (sum w d u, sum w d v, sum w d)
-  float su = 0.f, sv = 0.f, s1 = 0.f;
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    float wd = tp.w[k] * __ldg(d2img + tp.idx[k]);
-    su = fmaf(wd, tp.ux[k & 1], su);
-    sv = fmaf(wd, tp.uy[k >> 1], sv);
-    s1 += wd;
-  }
-  o.wd = s1;
-  mv(ps.Kinv, su, sv, s1, o.wpc[0], o.wpc[1], o.wpc[2]);
-  if (kNeedWorld) {
-    float rx, ry, rz;
-    ray_of(ps.M1, x, y, rx, ry, rz);
-    o.P1[0] = fmaf(d1, rx, ps.t1[0]);
-    o.P1[1] = fmaf(d1, ry, ps.t1[1]);
-    o.P1[2] = fmaf(d1, rz, ps.t1[2]);
-    // the four in-range bilinear weights sum to 1  =>  sum_k w_k (R2 p_k + t2) = R2 wpc + t2
-    mv(ps.R2, o.wpc[0], o.wpc[1], o.wpc[2], o.wP2[0], o.wP2[1], o.wP2[2]);
-    o.wP2[0] += ps.t2[0]; o.wP2[1] += ps.t2[1]; o.wP2[2] += ps.t2[2];
-  }
-  // p12 = R2^T (P1 + sf - t2) = d1 (A c) + cv + R2^T sf ;  i12 = K p12
-  float ax, ay, az, bx, by, bz;
-  ray_of(ps.A, x, y, ax, ay, az);
-  mtv(ps.R2, sfx, sfy, sfz, bx, by, bz);
-  o.p12[0] = fmaf(d1, ax, ps.cv[0]) + bx;
-  o.p12[1] = fmaf(d1, ay, ps.cv[1]) + by;
-  o.p12[2] = fmaf(d1, az, ps.cv[2]) + bz;
-  mv(ps.K, o.p12[0], o.p12[1], o.p12[2], o.i12[0], o.i12[1], o.i12[2]);
-  o.zok = !(o.i12[2] < 1e-3f);
-  o.rz = rcp_fast(o.i12[2] + 1e-8f);
-  if (o.zok) {
-    o.dflow[0] = o.i12[0] * o.rz - x;
-    o.dflow[1] = o.i12[1] * o.rz - y;
-  } else {
-    o.dflow[0] = 0.0f;
-    o.dflow[1] = 0.0f;
-  }
-}
-
 __device__ __forceinline__ float mask_of(const dvd_loss_cfg& c, float m2, float d1, float wz) {
-  float m = m2;
-  if (c.midas) {
-    m *= (d1 < 100.0f) ? 1.0f : 0.0f;
-    m *= (wz < 100.0f) ? 1.0f : 0.0f;
-  }
-  return m;
+  return (!c.midas || (d1 < 100.0f && wz < 100.0f)) ? m2 : 0.0f;
 }
 
 __device__ __forceinline__ float disp_term(const dvd_loss_cfg& c, float za, float zb) {
@@ -193,13 +75,13 @@ __device__ __forceinline__ float disp_term(const dvd_loss_cfg& c, float za, floa
   return fabsf(za - zb);
 }
 
-// ---------------------------------------------------------------------------------------------
-// vector access helpers: VEC consecutive pixels along x per thread
-template <int VEC> struct VecT;
-template <> struct VecT<1> { using T = float;  using F = float2; };
-template <> struct VecT<2> { using T = float2; using F = float4; };
-template <> struct VecT<4> { using T = float4; using F = float4; };
+// c * sign(v) (0 at v == 0)
+__device__ __forceinline__ float sgn_scale(float v, float c) {
+  return v == 0.f ? 0.f : __uint_as_float(__float_as_uint(c) ^ (__float_as_uint(v) & 0x80000000u));   // one LOP3
+}
 
+// ---------------------------------------------------------------------------------------------
+// vector access helpers (un-project kernels): VEC consecutive pixels along x per thread
 template <int VEC>
 __device__ __forceinline__ void load_vec(const float* __restrict__ p, float (&v)[VEC]) {
   if (VEC == 4) {
@@ -222,37 +104,33 @@ __device__ __forceinline__ void store_vec(float* __restrict__ p, const float (&v
     *p = v[0];
   }
 }
-template <int VEC>
-__device__ __forceinline__ void load_flow(const float* __restrict__ p, float (&fx)[VEC], float (&fy)[VEC]) {
-  // p points at flow[b,y,x,0]; 2*VEC consecutive floats
-  if (VEC == 4) {
-    float4 a = ldg_stream4(p), b = ldg_stream4(p + 4);
-    fx[0] = a.x; fy[0] = a.y; fx[1] = a.z; fy[1] = a.w;
-    fx[2] = b.x; fy[2] = b.y; fx[3] = b.z; fy[3] = b.w;
-  } else if (VEC == 2) {
-    float4 a = ldg_stream4(p);
-    fx[0] = a.x; fy[0] = a.y; fx[1] = a.z; fy[1] = a.w;
-  } else {
-    float2 a = __ldg(reinterpret_cast<const float2*>(p));
-    fx[0] = a.x; fy[0] = a.y;
-  }
-}
 
 constexpr int kThreads = 256;
 
 // ---------------------------------------------------------------------------------------------
 // un-project forward / adjoint
+
+// Kinv, R_which and t_which of pair b, straight from its [48]-float pose block
+__device__ __forceinline__ void load_camera(const float* __restrict__ poses, int b, int which, float* Kinv, float* R,
+                                            float* t) {
+  const float* p = poses + (size_t)b * DVD_POSE_STRIDE;
+  const int i = threadIdx.x;
+  if (i < 9) {
+    Kinv[i] = __ldg(p + i);
+    R[i] = __ldg(p + (which == 1 ? 18 : 27) + i);
+  }
+  if (i < 3) t[i] = __ldg(p + (which == 1 ? 36 : 39) + i);
+  __syncthreads();
+}
+
 template <int VEC>
 __global__ void __launch_bounds__(kThreads) unproject_fwd_kernel(const float* __restrict__ depth,
                                                                  const float* __restrict__ poses,
                                                                  float* __restrict__ P, int H, int W, int which) {
   DVD_PDL_ENTER();
-  __shared__ Pose ps;
+  __shared__ float Kinv[9], R[9], t[3];
   const int b = blockIdx.y;
-  load_pose(ps, poses, b);
-  __syncthreads();
-  const float* R = which == 1 ? ps.R1 : ps.R2;
-  const float* t = which == 1 ? ps.t1 : ps.t2;
+  load_camera(poses, b, which, Kinv, R, t);
   const int HW = H * W, items = HW / VEC, Wv = W / VEC;
   // (y, xv) walk of the grid-stride loop without a per-iteration integer division
   const int stride = gridDim.x * blockDim.x, sdy = stride / Wv, sdx = stride - sdy * Wv;
@@ -267,7 +145,7 @@ __global__ void __launch_bounds__(kThreads) unproject_fwd_kernel(const float* __
 #pragma unroll
     for (int v = 0; v < VEC; ++v) {
       float rx, ry, rz;
-      ray_of(ps.Kinv, (float)(x0 + v), (float)y, rx, ry, rz);
+      ray_of(Kinv, (float)(x0 + v), (float)y, rx, ry, rz);
       mv(R, d[v] * rx, d[v] * ry, d[v] * rz, ox[v], oy[v], oz[v]);
       ox[v] += t[0]; oy[v] += t[1]; oz[v] += t[2];
     }
@@ -283,11 +161,9 @@ __global__ void __launch_bounds__(kThreads) unproject_bwd_kernel(const float* __
                                                                  const float* __restrict__ poses,
                                                                  float* __restrict__ gd, int H, int W, int which) {
   DVD_PDL_ENTER();
-  __shared__ Pose ps;
+  __shared__ float Kinv[9], R[9], t[3];
   const int b = blockIdx.y;
-  load_pose(ps, poses, b);
-  __syncthreads();
-  const float* R = which == 1 ? ps.R1 : ps.R2;
+  load_camera(poses, b, which, Kinv, R, t);
   const int HW = H * W, items = HW / VEC, Wv = W / VEC;
   // (y, xv) walk of the grid-stride loop without a per-iteration integer division
   const int stride = gridDim.x * blockDim.x, sdy = stride / Wv, sdx = stride - sdy * Wv;
@@ -305,7 +181,7 @@ __global__ void __launch_bounds__(kThreads) unproject_bwd_kernel(const float* __
 #pragma unroll
     for (int v = 0; v < VEC; ++v) {
       float rx, ry, rz, wx, wy, wz;
-      ray_of(ps.Kinv, (float)(x0 + v), (float)y, rx, ry, rz);
+      ray_of(Kinv, (float)(x0 + v), (float)y, rx, ry, rz);
       mv(R, rx, ry, rz, wx, wy, wz);  // dP/dd = R * ray
       o[v] = fmaf(gz[v], wz, fmaf(gy[v], wy, gx[v] * wx));
     }
@@ -314,64 +190,399 @@ __global__ void __launch_bounds__(kThreads) unproject_bwd_kernel(const float* __
 }
 
 // ---------------------------------------------------------------------------------------------
-// fused forward: loss partial sums only
-template <int VEC, int MINB>
-__global__ void __launch_bounds__(kThreads, MINB) reproject_loss_fwd_kernel(
-    const float* __restrict__ depth_1, const float* __restrict__ depth_2, const float* __restrict__ flow,
-    const float* __restrict__ mask_2, const float* __restrict__ sf, const float* __restrict__ poses,
-    dvd_loss_cfg cfg, float* __restrict__ partials, int H, int W) {
-  DVD_PDL_ENTER();
-  __shared__ Pose ps;
-  __shared__ float red[kThreads / 32][4];
-  const int b = blockIdx.y;
-  load_pose(ps, poses, b);
-  __syncthreads();
-  const int HW = H * W, items = HW / VEC, Wv = W / VEC;
-  const float* d2img = depth_2 + (size_t)b * HW;
-  float s_flow = 0.f, s_disp = 0.f, s_sf = 0.f, s_m = 0.f;
-  // (y, xv) walk of the grid-stride loop without a per-iteration integer division
-  const int stride = gridDim.x * blockDim.x, sdy = stride / Wv, sdx = stride - sdy * Wv;
-  int it = blockIdx.x * blockDim.x + threadIdx.x;
-  int y = it / Wv, xv = it - y * Wv;
-  for (; it < items; it += stride, y += sdy, xv += sdx) {
-    if (xv >= Wv) { xv -= Wv; ++y; }
-    const int x0 = xv * VEC;
-    size_t pix = (size_t)y * W + x0;
-    float d1[VEC], m2[VEC], sx[VEC], sy[VEC], sz[VEC], fx[VEC], fy[VEC];
-    load_vec<VEC>(depth_1 + (size_t)b * HW + pix, d1);
-    load_vec<VEC>(mask_2 + (size_t)b * HW + pix, m2);
-    const float* sfp = sf + (size_t)b * 3 * HW + pix;
-    load_vec<VEC>(sfp, sx);
-    load_vec<VEC>(sfp + HW, sy);
-    load_vec<VEC>(sfp + 2 * (size_t)HW, sz);
-    load_flow<VEC>(flow + ((size_t)b * HW + pix) * 2, fx, fy);
-#pragma unroll
-    for (int v = 0; v < VEC; ++v) {
-      float x = (float)(x0 + v), yf = (float)y;
-      Taps tp = make_taps(x + fx[v], yf + fy[v], H, W);
-      Px o;
-      forward_px<true>(ps, d2img, tp, x, yf, d1[v], sx[v], sy[v], sz[v], o);
-      float m = mask_of(cfg, m2[v], d1[v], o.wpc[2]);
-      float ex = o.dflow[0] - fx[v], ey = o.dflow[1] - fy[v];
-      float fl = cfg.warm ? (ex * ex + ey * ey) : (fabsf(ex) + fabsf(ey));
-      float dl = disp_term(cfg, o.p12[2], o.wpc[2]);
-      float sl = fabsf(o.wP2[0] - o.P1[0] - sx[v]) + fabsf(o.wP2[1] - o.P1[1] - sy[v]) +
-                 fabsf(o.wP2[2] - o.P1[2] - sz[v]);
-      s_flow = fmaf(m, fl, s_flow);
-      s_disp = fmaf(m, dl, s_disp);
-      s_sf = fmaf(m, sl, s_sf);
-      s_m += m;
-    }
+// Poses of the loss and materialise kernels: derived once per call by pose_prep_kernel and copied into a __constant__ slot
+// with a device-to-device cudaMemcpyToSymbolAsync on the caller's stream (no host round trip). The kernels read every
+// entry as a broadcast operand straight from the constant bank.
+struct __align__(16) PoseC {
+  float Kinv[9];   //  0
+  float K[9];      //  9
+  float R2[9];     // 18
+  float nM1[9];    // 27  -(R1 Kinv)                 -(P1 - t1) = d1 * (nM1 c)
+  float A[9];      // 36  R2^T R1 Kinv               p12 = d1 * (A c) + cv + R2^T sf
+  float cv[3];     // 45  R2^T (t1 - t2)
+  float t21[3];    // 48  t2 - t1                    warped_global_p2 - P1 = R2 wpc + t21 + d1 * (nM1 c)
+  float t1[3];     // 51
+  float t2[3];     // 54
+  float pad[7];
+};
+static_assert(sizeof(PoseC) == 256, "PoseC layout");
+constexpr int kPoseSlots = 3;    // rotating slots: calls in flight on different streams do not share a slot
+constexpr int kPosePairs = 64;   // pairs per launch (larger batches are processed in chunks)
+__constant__ PoseC c_pose[kPoseSlots][kPosePairs];
+__device__ PoseC g_pose_stage[kPoseSlots][kPosePairs];
+
+// PoseC of one pair from its raw [48]-float pose block
+__device__ __forceinline__ void derive_pose(const float* __restrict__ p, PoseC& o) {
+  float Kinv[9], R1[9], R2[9], M1[9], t1[3], t2[3];
+  for (int i = 0; i < 9; ++i) {
+    Kinv[i] = p[i]; R1[i] = p[18 + i]; R2[i] = p[27 + i];
+    o.Kinv[i] = Kinv[i]; o.K[i] = p[9 + i]; o.R2[i] = R2[i];
   }
-  s_flow = warp_sum(s_flow); s_disp = warp_sum(s_disp); s_sf = warp_sum(s_sf); s_m = warp_sum(s_m);
-  const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) { red[wid][0] = s_flow; red[wid][1] = s_disp; red[wid][2] = s_sf; red[wid][3] = s_m; }
+  for (int i = 0; i < 3; ++i) { t1[i] = p[36 + i]; t2[i] = p[39 + i]; }
+  mm3(R1, Kinv, M1, false);
+  mm3(R2, M1, o.A, true);
+  for (int i = 0; i < 9; ++i) o.nM1[i] = -M1[i];
+  const float dx = t1[0] - t2[0], dy = t1[1] - t2[1], dz = t1[2] - t2[2];
+  for (int i = 0; i < 3; ++i) {
+    o.cv[i] = fmaf(R2[6 + i], dz, fmaf(R2[3 + i], dy, R2[i] * dx));
+    o.t21[i] = t2[i] - t1[i];
+    o.t1[i] = t1[i];
+    o.t2[i] = t2[i];
+  }
+}
+
+__global__ void pose_prep_kernel(const float* __restrict__ poses, int B, int slot) {
+  DVD_PDL_ENTER();
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B) derive_pose(poses + (size_t)b * DVD_POSE_STRIDE, g_pose_stage[slot][b]);
+}
+
+// The kernels with one grid row per pair (generic loss, materialise) derive their pair's PoseC once per CTA into shared
+// memory: at one or a few pairs per call, staging constant-bank poses would cost more than the loss kernel itself.
+__device__ __forceinline__ const PoseC& block_pose(const float* __restrict__ poses, int b) {
+  __shared__ PoseC ps;
+  if (threadIdx.x == 0) derive_pose(poses + (size_t)b * DVD_POSE_STRIDE, ps);
   __syncthreads();
-  if (threadIdx.x < 4) {
-    float a = 0.f;
+  return ps;
+}
+
+// ---------------------------------------------------------------------------------------------
+// The per-pixel chain, shared by every loss and materialise kernel. Column-vector algebra, c = (x, y, 1)^T.
+
+// streamed inputs of one pixel
+struct PixIn {
+  float d1, m2, sf[3], fx, fy;
+};
+
+// A c and nM1 c, c = (x, y, 1), split into the column-0 term and the part shared by the pixels of row y
+struct RowTerms {
+  float ra[3];   // A[:,1] y + A[:,2]
+  float rn[3];   // nM1[:,1] y + nM1[:,2]
+};
+__device__ __forceinline__ RowTerms row_terms(const PoseC& ps, float y) {
+  RowTerms r;
 #pragma unroll
-    for (int w = 0; w < kThreads / 32; ++w) a += red[w][threadIdx.x];
-    partials[((size_t)b * gridDim.x + blockIdx.x) * 4 + threadIdx.x] = a;
+  for (int k = 0; k < 3; ++k) {
+    r.ra[k] = fmaf(ps.A[3 * k + 1], y, ps.A[3 * k + 2]);
+    r.rn[k] = fmaf(ps.nM1[3 * k + 1], y, ps.nM1[3 * k + 2]);
+  }
+  return r;
+}
+
+// forward chain of one pixel
+struct PixFwd {
+  int i00, sx1, sy1;      // nw tap index; element offsets to the ne / sw taps (0 where clamped by the border)
+  float w[4];             // bilinear weights; a tap clamped by the border has weight exactly 0
+  float x0f, y0f;         // tap origin (the ne / sw / se taps sit at +1 wherever their weight is non-zero)
+  float s1;               // sum_k w_k d2_k = depth_warp_1_2
+  float wpc[3], p12[3], i12[3], rz;
+  float ex, ey;           // dflow_1_2 - flow_1_2 (zero flow substituted where the projection is rejected)
+  bool zok;               // i12.z >= 1e-3 (projection used; otherwise own coordinate, zero gradient)
+};
+
+// Bilinear taps follow ATen grid_sampler_2d(bilinear, padding_mode=border, align_corners=True) at the pixel coordinate
+// c + flow. The reference normalises to [-1,1] (losses/...:107-110) and ATen un-normalises again; that round trip is the
+// identity up to ~1e-7 relative (4e-5 px at W=384), far below the 1e-3 parity bar, so it is skipped.
+__device__ __forceinline__ void pixel_forward(const PoseC& ps, const float* __restrict__ d2img, int H, int W, float x,
+                                              float y, const RowTerms& rt, const PixIn& in, PixFwd& o) {
+  const float hw = (float)(W - 1), hh = (float)(H - 1);
+  const float nx = -x;
+  const float nqx = fmaf(in.fx, -1.0f, nx);   // -(x + flow_x)
+  const float nqy = fmaf(in.fy, -1.0f, -y);   // -(y + flow_y)
+  const float ix = fminf(hw, fmaxf(-nqx, 0.0f)), iy = fminf(hh, fmaxf(-nqy, 0.0f));
+  o.x0f = floorf(ix);
+  o.y0f = floorf(iy);
+  const int xi = (int)o.x0f, yi = (int)o.y0f;
+  o.i00 = yi * W + xi;
+  o.sx1 = xi < W - 1 ? 1 : 0;
+  o.sy1 = yi < H - 1 ? W : 0;
+  const float* q = d2img + o.i00;   // one 64-bit address per pixel, the other taps at small element offsets from it
+  const float dk0 = __ldg(q), dk1 = __ldg(q + o.sx1), dk2 = __ldg(q + o.sy1), dk3 = __ldg(q + o.sy1 + o.sx1);
+  // ---- arithmetic that does not depend on the gathered taps first: it runs while the gather is in flight ----
+  // p12 = d1 (A c) + cv + R2^T sf
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const float ac = fmaf(-ps.A[3 * k], nx, rt.ra[k]);
+    float t = fmaf(in.d1, ac, ps.cv[k]);
+    t = fmaf(ps.R2[k], in.sf[0], t);
+    t = fmaf(ps.R2[3 + k], in.sf[1], t);
+    o.p12[k] = fmaf(ps.R2[6 + k], in.sf[2], t);
+  }
+  mv(ps.K, o.p12[0], o.p12[1], o.p12[2], o.i12[0], o.i12[1], o.i12[2]);
+  o.rz = rcp_fast(__fadd_rn(o.i12[2], 1e-8f));
+  o.zok = !(o.i12[2] < 1e-3f);
+  // dflow - flow = i12.xy * rz - (c.xy + flow)
+  o.ex = o.zok ? fmaf(o.i12[0], o.rz, nqx) : -in.fx;
+  o.ey = o.zok ? fmaf(o.i12[1], o.rz, nqy) : -in.fy;
+  // clamped coordinate == W-1 (H-1) implies a zero fractional part, so the clamped taps need no explicit masking
+  const float wx1 = fmaf(o.x0f, -1.0f, ix), wy1 = fmaf(o.y0f, -1.0f, iy);
+  const float wx0 = fmaf(wx1, -1.0f, 1.0f), wy0 = fmaf(wy1, -1.0f, 1.0f);
+  o.w[0] = __fmul_rn(wx0, wy0); o.w[1] = __fmul_rn(wx1, wy0); o.w[2] = __fmul_rn(wx0, wy1); o.w[3] = __fmul_rn(wx1, wy1);
+  // ---- gathered taps ----
+  // wpc = sum_k w_k d2_k Kinv (u_k, v_k, 1) = Kinv (su, sv, s1), u_k = x0f (+1), v_k = y0f (+1)
+  const float wd0 = __fmul_rn(o.w[0], dk0), wd1 = __fmul_rn(o.w[1], dk1);
+  const float wd2 = __fmul_rn(o.w[2], dk2), wd3 = __fmul_rn(o.w[3], dk3);
+  const float eb = __fadd_rn(wd1, wd3), sb = __fadd_rn(wd2, wd3);
+  o.s1 = __fadd_rn(__fadd_rn(wd0, wd1), sb);
+  const float su = fmaf(o.x0f, o.s1, eb), sv = fmaf(o.y0f, o.s1, sb);
+  mv(ps.Kinv, su, sv, o.s1, o.wpc[0], o.wpc[1], o.wpc[2]);
+}
+
+// residual of the sf term: warped_global_p2 - P1 - sf = R2 wpc + t21 + d1 (nM1 c) - sf
+__device__ __forceinline__ void sf_residual(const PoseC& ps, float x, const RowTerms& rt, const PixIn& in,
+                                            const PixFwd& o, float (&e)[3]) {
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const float nr = fmaf(-ps.nM1[3 * k], -x, rt.rn[k]);   // -(M1 c)_k
+    const float t = fmaf(in.sf[k], -1.0f, fmaf(in.d1, nr, ps.t21[k]));
+    e[k] = fmaf(ps.R2[3 * k + 2], o.wpc[2], fmaf(ps.R2[3 * k + 1], o.wpc[1], fmaf(ps.R2[3 * k], o.wpc[0], t)));
+  }
+}
+
+// g_d2_k = w_k (hu u_k + hv v_k + h1), (u_k, v_k) = (x0f, y0f) (+1): the scatter of Kinv^T g_wpc = (hu, hv, h1)
+__device__ __forceinline__ void tap_grads(const PixFwd& o, float hu, float hv, float h1, float (&g)[4]) {
+  const float base = fmaf(hu, o.x0f, fmaf(hv, o.y0f, h1));
+  const float bx = __fadd_rn(base, hu);
+  g[0] = __fmul_rn(o.w[0], base);
+  g[1] = __fmul_rn(o.w[1], bx);
+  g[2] = __fmul_rn(o.w[2], __fadd_rn(base, hv));
+  g[3] = __fmul_rn(o.w[3], __fadd_rn(bx, hv));
+}
+
+struct LossSums {
+  float flow = 0.f, disp = 0.f, sf = 0.f, m = 0.f;
+};
+
+// Adds the masked loss terms of the N pixels (x0 + j, y) to acc[j]. Each term is formed for all N pixels before the next,
+// so a loss-mode branch is taken once per term rather than once per pixel (with per-pixel branches the compiler spills
+// the staged forward at its 72-register budget).
+template <int N>
+__device__ __forceinline__ void add_losses(const PoseC& ps, const dvd_loss_cfg& cfg, const float* __restrict__ d2img,
+                                           int H, int W, int x0, float y, const PixIn (&in)[N], LossSums (&acc)[N]) {
+  const RowTerms rt = row_terms(ps, y);
+  PixFwd o[N];
+  float e[N][3], m[N], fl[N], dl[N], sl[N];
+#pragma unroll
+  for (int j = 0; j < N; ++j) {
+    pixel_forward(ps, d2img, H, W, (float)(x0 + j), y, rt, in[j], o[j]);
+    sf_residual(ps, (float)(x0 + j), rt, in[j], o[j], e[j]);
+  }
+#pragma unroll
+  for (int j = 0; j < N; ++j) m[j] = mask_of(cfg, in[j].m2, in[j].d1, o[j].wpc[2]);
+  if (cfg.warm) {
+#pragma unroll
+    for (int j = 0; j < N; ++j) fl[j] = fmaf(o[j].ex, o[j].ex, __fmul_rn(o[j].ey, o[j].ey));
+  } else {
+#pragma unroll
+    for (int j = 0; j < N; ++j) fl[j] = fabsf(o[j].ex) + fabsf(o[j].ey);
+  }
+#pragma unroll
+  for (int j = 0; j < N; ++j) dl[j] = disp_term(cfg, o[j].p12[2], o[j].wpc[2]);
+#pragma unroll
+  for (int j = 0; j < N; ++j) sl[j] = fabsf(e[j][0]) + fabsf(e[j][1]) + fabsf(e[j][2]);
+#pragma unroll
+  for (int j = 0; j < N; ++j) {
+    acc[j].flow = fmaf(m[j], fl[j], acc[j].flow);
+    acc[j].disp = fmaf(m[j], dl[j], acc[j].disp);
+    acc[j].sf = fmaf(m[j], sl[j], acc[j].sf);
+    acc[j].m = __fadd_rn(acc[j].m, m[j]);
+  }
+}
+
+// backward of one pixel: g_(P1 + sf) -> gv, Kinv^T g_warped_p2_camera_2 -> h (tap_grads turns h into the gradients of
+// the four depth_2 taps in o)
+__device__ __forceinline__ void pixel_backward(const PoseC& ps, const dvd_loss_cfg& cfg, const float* __restrict__ d2img,
+                                               int H, int W, float x, float y, const RowTerms& rt, const PixIn& in,
+                                               float cf, float cd, PixFwd& o, float (&gv)[3], float (&h)[3]) {
+  pixel_forward(ps, d2img, H, W, x, y, rt, in, o);
+  const float m = mask_of(cfg, in.m2, in.d1, o.wpc[2]);
+  // --- flow term -> g_i12 (zero where the projection was rejected)
+  const float mcf = o.zok ? m * cf : 0.f;
+  float gux, guy;
+  if (cfg.warm) {
+    const float t2 = __fadd_rn(mcf, mcf);
+    gux = __fmul_rn(t2, o.ex); guy = __fmul_rn(t2, o.ey);
+  } else {
+    gux = sgn_scale(o.ex, mcf); guy = sgn_scale(o.ey, mcf);
+  }
+  const float gi0 = __fmul_rn(gux, o.rz), gi1 = __fmul_rn(guy, o.rz);
+  const float tt = fmaf(gux, o.i12[0], __fmul_rn(guy, o.i12[1]));
+  const float gi2 = __fmul_rn(__fmul_rn(tt, o.rz), __fmul_rn(o.rz, -1.0f));
+  float gp0, gp1, gp2;   // g_p12 = K^T g_i12
+  mtv(ps.K, gi0, gi1, gi2, gp0, gp1, gp2);
+  float hu, hv, h1;      // Kinv^T g_warped_p2_camera_2
+  float ge[3] = {0.f, 0.f, 0.f};
+  const float mc = __fmul_rn(m, cd);
+  if (cfg.second_is_disp) {
+    const float za = o.p12[2], zb = o.wpc[2];
+    float gwc2;
+    if (cfg.disp_mode == 0) {
+      const float ra = rcp_fast(fmaxf(za, 1e-3f)), rb = rcp_fast(fmaxf(zb, 1e-3f));
+      const float s = sgn_scale(fmaf(rb, -1.0f, ra), __fmul_rn(mc, 100.0f));
+      const float sa = za >= 1e-3f ? s : 0.f, sb = zb >= 1e-3f ? s : 0.f;
+      gp2 = fmaf(__fmul_rn(sa, ra), __fmul_rn(ra, -1.0f), gp2);
+      gwc2 = __fmul_rn(__fmul_rn(sb, rb), rb);
+    } else if (cfg.disp_mode == 1) {
+      // max(a,b)/min(a,b) - 1
+      const float a = fmaxf(za, 1e-3f), bb = fmaxf(zb, 1e-3f);
+      const float ra = rcp_fast(a), rb = rcp_fast(bb);
+      float ga, gb;
+      if (a >= bb) { ga = rb; gb = -a * rb * rb; }
+      else         { ga = -bb * ra * ra; gb = ra; }
+      gp2 = __fadd_rn(gp2, za >= 1e-3f ? ga * mc : 0.f);
+      gwc2 = zb >= 1e-3f ? gb * mc : 0.f;
+    } else {
+      const float s = sgn_scale(fmaf(zb, -1.0f, za), mc);
+      gp2 = __fadd_rn(gp2, s);
+      gwc2 = __fmul_rn(s, -1.0f);
+    }
+    hu = __fmul_rn(ps.Kinv[6], gwc2); hv = __fmul_rn(ps.Kinv[7], gwc2); h1 = __fmul_rn(ps.Kinv[8], gwc2);
+  } else {
+    float e[3];
+    sf_residual(ps, x, rt, in, o, e);
+    ge[0] = sgn_scale(e[0], mc); ge[1] = sgn_scale(e[1], mc); ge[2] = sgn_scale(e[2], mc);
+    // warped_global_p2 = R2 wpc + t2  =>  g_wpc = R2^T g_e
+    float a0, a1, a2;
+    mtv(ps.R2, ge[0], ge[1], ge[2], a0, a1, a2);
+    mtv(ps.Kinv, a0, a1, a2, hu, hv, h1);
+  }
+  // g_(P1 + sf) = R2 g_p12 ; the sf term adds -g_e to both P1 and sf
+  mv(ps.R2, gp0, gp1, gp2, gv[0], gv[1], gv[2]);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) gv[k] = fmaf(ge[k], -1.0f, gv[k]);
+  h[0] = hu; h[1] = hv; h[2] = h1;
+}
+
+// ---------------------------------------------------------------------------------------------
+// scatter-add of the four tap gradients of one pixel into g_depth_2 (q = &g_depth_2[i00])
+__device__ __forceinline__ void scatter4_atomic(float* q, int sx1, int sy1, const float (&g)[4]) {
+  if (g[0] != 0.f) atomicAdd(q, g[0]);
+  if (g[1] != 0.f) atomicAdd(q + sx1, g[1]);
+  if (g[2] != 0.f) atomicAdd(q + sy1, g[2]);
+  if (g[3] != 0.f) atomicAdd(q + sy1 + sx1, g[3]);
+}
+__device__ __forceinline__ void red_global_v2(float* p, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
+}
+__device__ __forceinline__ void red_global_v4(float* p, float a, float b, float c, float d) {
+  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+}
+// Vector form: needs W % 4 == 0 and a 16-byte aligned g_depth_2 image. Whenever the nw tap sits on an even column the
+// (nw, ne) and (sw, se) taps are two 8-byte aligned pairs: one vector reduction each.
+__device__ __forceinline__ void scatter4_vec(float* q, int i00, int sx1, int sy1, const float (&g)[4]) {
+  if (((i00 & 1) == 0) && sx1 == 1) {
+    if (g[0] != 0.f || g[1] != 0.f) red_global_v2(q, g[0], g[1]);
+    if (g[2] != 0.f || g[3] != 0.f) {
+      if (sy1 != 0) red_global_v2(q + sy1, g[2], g[3]);
+      else red_global_v2(q, g[2], g[3]);     // clamped bottom row: both weights are exactly 0 here, kept for form
+    }
+  } else if (((i00 & 3) == 1) && sx1 == 1) {
+    // odd column whose pair still lies inside one 16-byte quad: one 4-wide reduction {0, g, g, 0} per row instead of two
+    // scalar ones (the LSU's reduction rate is per active lane, not per byte: DESIGN.md 8)
+    if (g[0] != 0.f || g[1] != 0.f) red_global_v4(q - 1, 0.f, g[0], g[1], 0.f);
+    if (g[2] != 0.f || g[3] != 0.f) red_global_v4(q - 1 + sy1, 0.f, g[2], g[3], 0.f);
+  } else {
+    scatter4_atomic(q, sx1, sy1, g);
+  }
+}
+
+// per-block partial sums -> out[0..3]; every thread of a kThreads-thread group must call it (named barrier 1, so a
+// producer warp that has already exited does not take part)
+__device__ __forceinline__ void write_block_sums(const LossSums& a, float* __restrict__ out) {
+  __shared__ float red[kThreads / 32][4];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const float s_flow = warp_sum(a.flow), s_disp = warp_sum(a.disp), s_sf = warp_sum(a.sf), s_m = warp_sum(a.m);
+  if (lane == 0) { red[warp][0] = s_flow; red[warp][1] = s_disp; red[warp][2] = s_sf; red[warp][3] = s_m; }
+  asm volatile("bar.sync 1, %0;" ::"n"(kThreads) : "memory");
+  if (threadIdx.x < 4) {
+    float s = 0.f;
+#pragma unroll
+    for (int w = 0; w < kThreads / 32; ++w) s += red[w][threadIdx.x];
+    out[threadIdx.x] = s;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Generic loss kernels: any W and alignment, scalar loads, blockIdx.y is the pair. The forward walks N x-adjacent pixels
+// per thread and grid-stride step (N = 2 when W is even, so a pair never straddles a row, as in the staged consumer;
+// N = 1 otherwise). The scatter-add backward runs one pixel per thread: more warps in flight hide the atomic latency.
+
+__device__ __forceinline__ PixIn load_pixel(const float* __restrict__ depth_1, const float* __restrict__ mask_2,
+                                            const float* __restrict__ sf, const float* __restrict__ flow, size_t b,
+                                            int HW, int p) {
+  const size_t i = b * HW + p;
+  PixIn in;
+  in.d1 = __ldg(depth_1 + i);
+  in.m2 = mask_2 ? __ldg(mask_2 + i) : 0.f;
+  const float* s = sf ? sf + b * 3 * HW + p : nullptr;
+  for (int k = 0; k < 3; ++k) in.sf[k] = s ? __ldg(s + (size_t)k * HW) : 0.f;
+  in.fx = __ldg(flow + 2 * i);
+  in.fy = __ldg(flow + 2 * i + 1);
+  return in;
+}
+
+// the per-pixel-slot accumulators of a thread, summed in slot order
+template <int N>
+__device__ __forceinline__ LossSums sum_slots(const LossSums (&acc)[N]) {
+  LossSums a = acc[0];
+#pragma unroll
+  for (int j = 1; j < N; ++j) {
+    a.flow += acc[j].flow;
+    a.disp += acc[j].disp;
+    a.sf += acc[j].sf;
+    a.m += acc[j].m;
+  }
+  return a;
+}
+
+template <int N>
+__global__ void __launch_bounds__(kThreads, 2) reproject_loss_fwd_kernel(
+    const float* __restrict__ depth_1, const float* __restrict__ depth_2, const float* __restrict__ flow,
+    const float* __restrict__ mask_2, const float* __restrict__ sf, dvd_loss_cfg cfg, float* __restrict__ partials,
+    int H, int W, const float* __restrict__ poses) {
+  DVD_PDL_ENTER();
+  const int HW = H * W;
+  const size_t b = blockIdx.y;
+  const PoseC& ps = block_pose(poses, blockIdx.y);
+  const float* d2img = depth_2 + b * HW;
+  LossSums acc[N];   // one per pixel slot
+  for (int p = (blockIdx.x * blockDim.x + threadIdx.x) * N; p < HW; p += gridDim.x * blockDim.x * N) {
+    const int y = p / W;
+    PixIn in[N];
+#pragma unroll
+    for (int j = 0; j < N; ++j) in[j] = load_pixel(depth_1, mask_2, sf, flow, b, HW, p + j);
+    add_losses<N>(ps, cfg, d2img, H, W, p - y * W, (float)y, in, acc);
+  }
+  write_block_sums(sum_slots(acc), partials + (b * gridDim.x + blockIdx.x) * 4);
+}
+
+__global__ void __launch_bounds__(kThreads) reproject_loss_bwd_kernel(
+    const float* __restrict__ depth_1, const float* __restrict__ depth_2, const float* __restrict__ flow,
+    const float* __restrict__ mask_2, const float* __restrict__ sf, dvd_loss_cfg cfg, const float* __restrict__ scalars,
+    float gscale, const float* __restrict__ gscale_dev, float* __restrict__ g_sf, float* __restrict__ g_d2, int H, int W,
+    const float* __restrict__ poses) {
+  DVD_PDL_ENTER();
+  const int HW = H * W;
+  const size_t b = blockIdx.y;
+  const PoseC& ps = block_pose(poses, blockIdx.y);
+  const float gs = gscale * (gscale_dev ? __ldg(gscale_dev) : 1.0f);
+  const float cf = __ldg(scalars + DVD_S_CF) * gs;
+  const float cd = __ldg(scalars + DVD_S_CD) * gs;
+  const float* d2img = depth_2 + b * HW;
+  float* gd2img = g_d2 ? g_d2 + b * HW : nullptr;
+  for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < HW; p += gridDim.x * blockDim.x) {
+    const int y = p / W;
+    PixFwd o;
+    float gv[3], h[3];
+    pixel_backward(ps, cfg, d2img, H, W, (float)(p - y * W), (float)y, row_terms(ps, (float)y),
+                   load_pixel(depth_1, mask_2, sf, flow, b, HW, p), cf, cd, o, gv, h);
+    float* gsp = g_sf + b * 3 * HW + p;
+    gsp[0] = gv[0]; gsp[HW] = gv[1]; gsp[2 * (size_t)HW] = gv[2];
+    if (gd2img) {
+      float gd[4];
+      tap_grads(o, h[0], h[1], h[2], gd);
+      scatter4_atomic(gd2img + o.i00, o.sx1, o.sy1, gd);
+    }
   }
 }
 
@@ -410,205 +621,212 @@ __global__ void __launch_bounds__(256) reproject_finalize_kernel(const float* __
 }
 
 // ---------------------------------------------------------------------------------------------
-// fused backward: g_sf (== g_global_p1) and scatter-add of g_depth_2
-__device__ __forceinline__ float sgn(float v) { return (v > 0.f) ? 1.f : ((v < 0.f) ? -1.f : 0.f); }
+// Staged loss kernels (W % 4 == 0, 16-byte aligned streamed inputs): the five streamed inputs (28 of the 32 bytes per
+// pixel) travel global -> shared memory as 1-D bulk async copies issued by a producer warp into a ring of kStages tiles,
+// completion on mbarriers; the kThreads consumer threads only see shared-memory latency for them, and the bytes in flight
+// per SM (CTAs x kStages x 14 KB) no longer depend on occupancy or on how the compiler schedules the loads. Each consumer
+// thread owns one x-adjacent pixel pair per tile. Only the bilinear gather of depth_2 is a global load, and g_depth_2 is
+// accumulated with global reductions; staging either through shared memory is a possible variant that has not been
+// measured on sm_90.
+constexpr int kStages = 4;
+constexpr int kTile = 2 * kThreads;                               // pixels per stage
+constexpr int kTileFloats = 7 * kTile;                            // d1, mask, sf.x, sf.y, sf.z, flow (2 floats per pixel)
+constexpr int kStagedSmem = kStages * kTileFloats * (int)sizeof(float);
+constexpr int kFwdCtasPerSm = 3, kBwdCtasPerSm = 2;
 
-template <int VEC>
-__global__ void __launch_bounds__(kThreads) reproject_loss_bwd_kernel(
-    const float* __restrict__ depth_1, const float* __restrict__ depth_2, const float* __restrict__ flow,
-    const float* __restrict__ mask_2, const float* __restrict__ sf, const float* __restrict__ poses,
-    dvd_loss_cfg cfg, const float* __restrict__ scalars, float gscale, const float* __restrict__ gscale_dev,
-    float* __restrict__ g_sf,
-    float* __restrict__ g_d2, int H, int W) {
-  DVD_PDL_ENTER();
-  __shared__ Pose ps;
-  const int b = blockIdx.y;
-  load_pose(ps, poses, b);
+// The producer warp streams tiles and returns false; each consumer thread calls consume(bl, p, in[2]) for its pixel pair
+// (p, p + 1) of pair bl of the chunk in every tile, then returns true. A chunk's pairs are split into tiles_per_pair tiles
+// each; CTAs walk the tiles with a stride of gridDim.x.
+template <class Consume>
+__device__ __forceinline__ bool staged_pairs(const float* __restrict__ depth_1, const float* __restrict__ mask_2,
+                                             const float* __restrict__ sf, const float* __restrict__ flow, int HW, int b0,
+                                             int nb, int tiles_per_pair, Consume&& consume) {
+  using namespace tc;
+  extern __shared__ __align__(128) float stage_mem[];
+  __shared__ uint64_t full[kStages], empty[kStages];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int ntiles = nb * tiles_per_pair;
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < kStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kThreads / 32); }
+    fence_mbar_init();
+  }
   __syncthreads();
+  if (warp == kThreads / 32) {
+    if (lane == 0) {
+      uint32_t it = 0;
+      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
+        const uint32_t s = it % kStages, ph = (it / kStages) & 1u;
+        mbar_wait(&empty[s], ph ^ 1u);
+        const int bl = tile / tiles_per_pair, p0 = (tile - bl * tiles_per_pair) * kTile;
+        const size_t b = (size_t)(b0 + bl);
+        float* dst = stage_mem + (size_t)s * kTileFloats;
+        const uint32_t n4 = (uint32_t)min(kTile, HW - p0) * 4u;
+        mbar_arrive_expect_tx(&full[s], n4 * 7u);
+        bulk_g2s(dst, depth_1 + b * HW + p0, n4, &full[s]);
+        bulk_g2s(dst + kTile, mask_2 + b * HW + p0, n4, &full[s]);
+        bulk_g2s(dst + 2 * kTile, sf + (b * 3 + 0) * HW + p0, n4, &full[s]);
+        bulk_g2s(dst + 3 * kTile, sf + (b * 3 + 1) * HW + p0, n4, &full[s]);
+        bulk_g2s(dst + 4 * kTile, sf + (b * 3 + 2) * HW + p0, n4, &full[s]);
+        bulk_g2s(dst + 5 * kTile, flow + (b * HW + p0) * 2, n4 * 2u, &full[s]);
+      }
+    }
+    return false;
+  }
+  const int tv = threadIdx.x * 2;
+  uint32_t it = 0;
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
+    const uint32_t s = it % kStages, ph = (it / kStages) & 1u;
+    mbar_wait(&full[s], ph);
+    const float* src = stage_mem + (size_t)s * kTileFloats + tv;
+    const float2 d1 = *reinterpret_cast<const float2*>(src), m2 = *reinterpret_cast<const float2*>(src + kTile);
+    const float2 sx = *reinterpret_cast<const float2*>(src + 2 * kTile);
+    const float2 sy = *reinterpret_cast<const float2*>(src + 3 * kTile);
+    const float2 sz = *reinterpret_cast<const float2*>(src + 4 * kTile);
+    const float4 f = *reinterpret_cast<const float4*>(src + 5 * kTile + tv);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[s]);     // values are in registers: hand the stage back
+    const int bl = tile / tiles_per_pair, p = (tile - bl * tiles_per_pair) * kTile + tv;
+    if (p >= HW) continue;
+    const PixIn in[2] = {{d1.x, m2.x, {sx.x, sy.x, sz.x}, f.x, f.y}, {d1.y, m2.y, {sx.y, sy.y, sz.y}, f.z, f.w}};
+    consume(bl, p, in);
+  }
+  return true;
+}
+
+__global__ void __launch_bounds__(kThreads + 32, kFwdCtasPerSm) reproject_loss_fwd_staged_kernel(
+    const float* __restrict__ depth_1, const float* __restrict__ depth_2, const float* __restrict__ flow,
+    const float* __restrict__ mask_2, const float* __restrict__ sf, dvd_loss_cfg cfg, float* __restrict__ partials,
+    int H, int W, int slot, int b0, int nb, int tiles_per_pair) {
+  DVD_PDL_ENTER();
+  const int HW = H * W;
+  LossSums acc[2];   // one per pixel slot of the pair
+  if (!staged_pairs(depth_1, mask_2, sf, flow, HW, b0, nb, tiles_per_pair, [&](int bl, int p, const PixIn (&in)[2]) {
+        const PoseC& ps = c_pose[slot][bl];
+        const float* d2img = depth_2 + (size_t)(b0 + bl) * HW;
+        const int y = p / W;
+        add_losses<2>(ps, cfg, d2img, H, W, p - y * W, (float)y, in, acc);
+      }))
+    return;
+  write_block_sums(sum_slots(acc), partials + (size_t)blockIdx.x * 4);
+}
+
+__global__ void __launch_bounds__(kThreads + 32, kBwdCtasPerSm) reproject_loss_bwd_staged_kernel(
+    const float* __restrict__ depth_1, const float* __restrict__ depth_2, const float* __restrict__ flow,
+    const float* __restrict__ mask_2, const float* __restrict__ sf, dvd_loss_cfg cfg, const float* __restrict__ scalars,
+    float gscale, const float* __restrict__ gscale_dev, float* __restrict__ g_sf, float* __restrict__ g_d2, int H, int W,
+    int slot, int b0, int nb, int tiles_per_pair) {
+  DVD_PDL_ENTER();
+  const int HW = H * W;
   const float gs = gscale * (gscale_dev ? __ldg(gscale_dev) : 1.0f);
   const float cf = __ldg(scalars + DVD_S_CF) * gs;
   const float cd = __ldg(scalars + DVD_S_CD) * gs;
-  const int HW = H * W, items = HW / VEC, Wv = W / VEC;
-  const float* d2img = depth_2 + (size_t)b * HW;
-  float* gd2img = g_d2 ? g_d2 + (size_t)b * HW : nullptr;
-  // (y, xv) walk of the grid-stride loop without a per-iteration integer division
-  const int stride = gridDim.x * blockDim.x, sdy = stride / Wv, sdx = stride - sdy * Wv;
-  int it = blockIdx.x * blockDim.x + threadIdx.x;
-  int y = it / Wv, xv = it - y * Wv;
-  for (; it < items; it += stride, y += sdy, xv += sdx) {
-    if (xv >= Wv) { xv -= Wv; ++y; }
-    const int x0 = xv * VEC;
-    size_t pix = (size_t)y * W + x0;
-    float d1[VEC], m2[VEC], sx[VEC], sy[VEC], sz[VEC], fx[VEC], fy[VEC];
-    float ox[VEC], oy[VEC], oz[VEC];
-    load_vec<VEC>(depth_1 + (size_t)b * HW + pix, d1);
-    load_vec<VEC>(mask_2 + (size_t)b * HW + pix, m2);
-    const float* sfp = sf + (size_t)b * 3 * HW + pix;
-    load_vec<VEC>(sfp, sx);
-    load_vec<VEC>(sfp + HW, sy);
-    load_vec<VEC>(sfp + 2 * (size_t)HW, sz);
-    load_flow<VEC>(flow + ((size_t)b * HW + pix) * 2, fx, fy);
+  staged_pairs(depth_1, mask_2, sf, flow, HW, b0, nb, tiles_per_pair, [&](int bl, int p, const PixIn (&in)[2]) {
+    const PoseC& ps = c_pose[slot][bl];
+    const size_t b = (size_t)(b0 + bl);
+    const float* d2img = depth_2 + b * HW;
+    float* gd2img = g_d2 ? g_d2 + b * HW : nullptr;
+    const int y = p / W, x0 = p - y * W;
+    const RowTerms rt = row_terms(ps, (float)y);
+    float gv[2][3];
 #pragma unroll
-    for (int v = 0; v < VEC; ++v) {
-      float x = (float)(x0 + v), yf = (float)y;
-      Taps tp = make_taps(x + fx[v], yf + fy[v], H, W);
-      Px o;
-      if (cfg.second_is_disp) forward_px<false>(ps, d2img, tp, x, yf, d1[v], sx[v], sy[v], sz[v], o);
-      else                    forward_px<true>(ps, d2img, tp, x, yf, d1[v], sx[v], sy[v], sz[v], o);
-      float m = mask_of(cfg, m2[v], d1[v], o.wpc[2]);
-      // --- gradient w.r.t. i12 = K p12 from the flow term
-      float gi0 = 0.f, gi1 = 0.f, gi2 = 0.f;
-      if (o.zok) {
-        float ex = o.dflow[0] - fx[v], ey = o.dflow[1] - fy[v];
-        float gux = cfg.warm ? 2.f * ex : sgn(ex);
-        float guy = cfg.warm ? 2.f * ey : sgn(ey);
-        gux *= m * cf; guy *= m * cf;
-        const float rz = o.rz;
-        gi0 = gux * rz;
-        gi1 = guy * rz;
-        gi2 = -(gux * o.i12[0] + guy * o.i12[1]) * rz * rz;
-      }
-      float gp0, gp1, gp2;  // g_p12 = K^T g_i12
-      mtv(ps.K, gi0, gi1, gi2, gp0, gp1, gp2);
-      float gwc0 = 0.f, gwc1 = 0.f, gwc2 = 0.f;  // g_warped_p2_camera_2
-      float ge0 = 0.f, ge1 = 0.f, ge2 = 0.f;     // g_(sf_by_depth - sf)
-      if (cfg.second_is_disp) {
-        float za = o.p12[2], zb = o.wpc[2];
-        float mc = m * cd;
-        if (cfg.disp_mode == 0) {
-          float a = fmaxf(za, 1e-3f), bb = fmaxf(zb, 1e-3f);
-          const float ra = rcp_fast(a), rb = rcp_fast(bb);
-          float s = 100.f * sgn(ra - rb) * mc;
-          if (za >= 1e-3f) gp2 -= s * ra * ra;
-          if (zb >= 1e-3f) gwc2 += s * rb * rb;
-        } else if (cfg.disp_mode == 1) {
-          float a = fmaxf(za, 1e-3f), bb = fmaxf(zb, 1e-3f);
-          // max(a,b)/min(a,b) - 1
-          float ga, gb;
-          const float ra = rcp_fast(a), rb = rcp_fast(bb);
-          if (a >= bb) { ga = rb; gb = -a * rb * rb; }
-          else         { ga = -bb * ra * ra; gb = ra; }
-          if (za >= 1e-3f) gp2 += ga * mc;
-          if (zb >= 1e-3f) gwc2 += gb * mc;
-        } else {
-          float s = sgn(za - zb) * mc;
-          gp2 += s;
-          gwc2 -= s;
-        }
-      } else {
-        float mc = m * cd;
-        ge0 = mc * sgn(o.wP2[0] - o.P1[0] - sx[v]);
-        ge1 = mc * sgn(o.wP2[1] - o.P1[1] - sy[v]);
-        ge2 = mc * sgn(o.wP2[2] - o.P1[2] - sz[v]);
-        // wP2 = sum_k w_k (R2 p2c2_k + t2)  =>  g_wpc += R2^T g_e
-        float a0, a1, a2;
-        mtv(ps.R2, ge0, ge1, ge2, a0, a1, a2);
-        gwc0 += a0; gwc1 += a1; gwc2 += a2;
-      }
-      // g_(P1 + sf) = R2 g_p12 ; sf_loss adds -g_e to both P1 and sf
-      float gv0, gv1, gv2;
-      mv(ps.R2, gp0, gp1, gp2, gv0, gv1, gv2);
-      ox[v] = gv0 - ge0; oy[v] = gv1 - ge1; oz[v] = gv2 - ge2;
-      // scatter to depth_2: wpc = Kinv (sum w d u, sum w d v, sum w d)  =>  g_d2_k = w_k (Kinv^T g_wpc).(u_k, v_k, 1)
+    for (int j = 0; j < 2; ++j) {
+      PixFwd o;
+      float h[3];
+      pixel_backward(ps, cfg, d2img, H, W, (float)(x0 + j), (float)y, rt, in[j], cf, cd, o, gv[j], h);
       if (gd2img) {
-        float hu, hv, h1;
-        mtv(ps.Kinv, gwc0, gwc1, gwc2, hu, hv, h1);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          float g = tp.w[k] * fmaf(hu, tp.ux[k & 1], fmaf(hv, tp.uy[k >> 1], h1));
-          if (g != 0.f) atomicAdd(gd2img + tp.idx[k], g);
-        }
+        float gd[4];
+        tap_grads(o, h[0], h[1], h[2], gd);
+        scatter4_vec(gd2img + o.i00, o.i00, o.sx1, o.sy1, gd);
       }
     }
-    float* gs = g_sf + (size_t)b * 3 * HW + pix;
-    store_vec<VEC>(gs, ox);
-    store_vec<VEC>(gs + HW, oy);
-    store_vec<VEC>(gs + 2 * (size_t)HW, oz);
-  }
+    float* gsp = g_sf + b * 3 * HW + p;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) *reinterpret_cast<float2*>(gsp + (size_t)k * HW) = make_float2(gv[0][k], gv[1][k]);
+  });
 }
 
 // ---------------------------------------------------------------------------------------------
 // materialise every per-pixel tensor of the two reference modules (not on the training fast path)
+__device__ __forceinline__ void st3(float* p, size_t o3, int HW, float a, float b, float c) {
+  if (p) { p[o3] = a; p[o3 + HW] = b; p[o3 + 2 * (size_t)HW] = c; }
+}
+__device__ __forceinline__ void ld3(const float* p, size_t o3, int HW, float& a, float& b, float& c) {
+  if (p) { a = p[o3]; b = p[o3 + HW]; c = p[o3 + 2 * (size_t)HW]; } else { a = b = c = 0.f; }
+}
+
 __global__ void __launch_bounds__(kThreads) reproject_materialize_kernel(
     const float* __restrict__ depth_1, const float* __restrict__ depth_2, const float* __restrict__ flow,
-    const float* __restrict__ sf, const float* __restrict__ poses, float* __restrict__ global_p1,
-    float* __restrict__ sf_by_depth, float* __restrict__ warped_global_p2, float* __restrict__ warped_p2_camera_2,
-    float* __restrict__ p1_camera_2, float* __restrict__ dflow, float* __restrict__ staticflow,
-    float* __restrict__ depth_image, float* __restrict__ depth_warp, int H, int W) {
+    const float* __restrict__ sf, float* __restrict__ global_p1, float* __restrict__ sf_by_depth,
+    float* __restrict__ warped_global_p2, float* __restrict__ warped_p2_camera_2, float* __restrict__ p1_camera_2,
+    float* __restrict__ dflow, float* __restrict__ staticflow, float* __restrict__ depth_image,
+    float* __restrict__ depth_warp, int H, int W, const float* __restrict__ poses) {
   DVD_PDL_ENTER();
-  __shared__ Pose ps;
-  const int b = blockIdx.y;
-  load_pose(ps, poses, b);
-  __syncthreads();
   const int HW = H * W;
-  const float* d2img = depth_2 + (size_t)b * HW;
+  const size_t b = blockIdx.y;
+  const PoseC& ps = block_pose(poses, blockIdx.y);
+  const float* d2img = depth_2 + b * HW;
   for (int pix = blockIdx.x * blockDim.x + threadIdx.x; pix < HW; pix += gridDim.x * blockDim.x) {
-    int y = pix / W, xi = pix - y * W;
-    float x = (float)xi, yf = (float)y;
-    float d1 = depth_1[(size_t)b * HW + pix];
-    float2 f = *reinterpret_cast<const float2*>(flow + ((size_t)b * HW + pix) * 2);
-    float sx = 0.f, sy = 0.f, sz = 0.f;
-    if (sf) {
-      const float* sfp = sf + (size_t)b * 3 * HW + pix;
-      sx = sfp[0]; sy = sfp[HW]; sz = sfp[2 * (size_t)HW];
+    const int y = pix / W;
+    const float x = (float)(pix - y * W), yf = (float)y;
+    const PixIn in = load_pixel(depth_1, nullptr, sf, flow, b, HW, pix);
+    const RowTerms rt = row_terms(ps, yf);
+    PixFwd o;
+    pixel_forward(ps, d2img, H, W, x, yf, rt, in, o);
+    // P1 = d1 (M1 c) + t1 ; warped_global_p2 = R2 wpc + t2 (the four in-range bilinear weights sum to 1)
+    float n[3], P1[3], wP2[3];
+    ray_of(ps.nM1, x, yf, n[0], n[1], n[2]);
+    mv(ps.R2, o.wpc[0], o.wpc[1], o.wpc[2], wP2[0], wP2[1], wP2[2]);
+    for (int k = 0; k < 3; ++k) {
+      P1[k] = fmaf(-in.d1, n[k], ps.t1[k]);
+      wP2[k] += ps.t2[k];
     }
-    Taps tp = make_taps(x + f.x, yf + f.y, H, W);
-    Px o, os;
-    forward_px<true>(ps, d2img, tp, x, yf, d1, sx, sy, sz, o);
-    size_t o3 = (size_t)b * 3 * HW + pix, o2 = (size_t)b * 2 * HW + pix, o1 = (size_t)b * HW + pix;
-    if (global_p1) { global_p1[o3] = o.P1[0]; global_p1[o3 + HW] = o.P1[1]; global_p1[o3 + 2 * (size_t)HW] = o.P1[2]; }
-    if (sf_by_depth) {
-      sf_by_depth[o3] = o.wP2[0] - o.P1[0];
-      sf_by_depth[o3 + HW] = o.wP2[1] - o.P1[1];
-      sf_by_depth[o3 + 2 * (size_t)HW] = o.wP2[2] - o.P1[2];
+    const size_t o3 = b * 3 * HW + pix, o2 = b * 2 * HW + pix, o1 = b * HW + pix;
+    st3(global_p1, o3, HW, P1[0], P1[1], P1[2]);
+    st3(sf_by_depth, o3, HW, wP2[0] - P1[0], wP2[1] - P1[1], wP2[2] - P1[2]);
+    st3(warped_global_p2, o3, HW, wP2[0], wP2[1], wP2[2]);
+    st3(warped_p2_camera_2, o3, HW, o.wpc[0], o.wpc[1], o.wpc[2]);
+    st3(p1_camera_2, o3, HW, o.p12[0], o.p12[1], o.p12[2]);
+    if (dflow) {
+      dflow[o2] = o.zok ? fmaf(o.i12[0], o.rz, -x) : 0.f;
+      dflow[o2 + HW] = o.zok ? fmaf(o.i12[1], o.rz, -yf) : 0.f;
     }
-    if (warped_global_p2) { warped_global_p2[o3] = o.wP2[0]; warped_global_p2[o3 + HW] = o.wP2[1]; warped_global_p2[o3 + 2 * (size_t)HW] = o.wP2[2]; }
-    if (warped_p2_camera_2) { warped_p2_camera_2[o3] = o.wpc[0]; warped_p2_camera_2[o3 + HW] = o.wpc[1]; warped_p2_camera_2[o3 + 2 * (size_t)HW] = o.wpc[2]; }
-    if (p1_camera_2) { p1_camera_2[o3] = o.p12[0]; p1_camera_2[o3 + HW] = o.p12[1]; p1_camera_2[o3 + 2 * (size_t)HW] = o.p12[2]; }
-    if (dflow) { dflow[o2] = o.dflow[0]; dflow[o2 + HW] = o.dflow[1]; }
     if (depth_image) depth_image[o1] = o.i12[2];
-    if (depth_warp) depth_warp[o1] = o.wd;
+    if (depth_warp) depth_warp[o1] = o.s1;
     if (staticflow) {
-      forward_px<false>(ps, d2img, tp, x, yf, d1, 0.f, 0.f, 0.f, os);
-      staticflow[o2] = os.dflow[0];
-      staticflow[o2 + HW] = os.dflow[1];
+      PixIn in0 = in;
+      in0.sf[0] = in0.sf[1] = in0.sf[2] = 0.f;
+      PixFwd os;
+      pixel_forward(ps, d2img, H, W, x, yf, rt, in0, os);
+      staticflow[o2] = os.zok ? fmaf(os.i12[0], os.rz, -x) : 0.f;
+      staticflow[o2 + HW] = os.zok ? fmaf(os.i12[1], os.rz, -yf) : 0.f;
     }
   }
 }
 
-// ---------------------------------------------------------------------------------------------
-// adjoint of reproject_materialize_kernel for ARBITRARY cotangents on its nine outputs (operator-level drop-in:
-// the mirrors of flow_by_depth / scene_flow_projection_slack stay differentiable for user-defined losses).
+// Adjoint of reproject_materialize_kernel for ARBITRARY cotangents on its nine outputs (operator-level drop-in: the mirrors
+// of flow_by_depth / scene_flow_projection_slack stay differentiable for user-defined losses).
 struct MatGrads {
   const float* global_p1; const float* sf_by_depth; const float* warped_global_p2; const float* warped_p2_camera_2;
   const float* p1_camera_2; const float* dflow; const float* staticflow; const float* depth_image; const float* depth_warp;
 };
-__device__ __forceinline__ void ld3(const float* p, size_t o3, int HW, float& a, float& b, float& c) {
-  if (p) { a = p[o3]; b = p[o3 + HW]; c = p[o3 + 2 * (size_t)HW]; } else { a = b = c = 0.f; }
-}
 __global__ void __launch_bounds__(kThreads) reproject_materialize_bwd_kernel(
     const float* __restrict__ depth_1, const float* __restrict__ depth_2, const float* __restrict__ flow,
-    const float* __restrict__ sf, const float* __restrict__ poses, MatGrads G, float* __restrict__ g_d1,
-    float* __restrict__ g_d2, float* __restrict__ g_sf, int H, int W) {
+    const float* __restrict__ sf, MatGrads G, float* __restrict__ g_d1, float* __restrict__ g_d2,
+    float* __restrict__ g_sf, int H, int W, const float* __restrict__ poses) {
   DVD_PDL_ENTER();
-  __shared__ Pose ps;
-  const int b = blockIdx.y;
-  load_pose(ps, poses, b);
-  __syncthreads();
   const int HW = H * W;
-  const float* d2img = depth_2 + (size_t)b * HW;
+  const size_t b = blockIdx.y;
+  const PoseC& ps = block_pose(poses, blockIdx.y);
+  const float* d2img = depth_2 + b * HW;
   for (int pix = blockIdx.x * blockDim.x + threadIdx.x; pix < HW; pix += gridDim.x * blockDim.x) {
-    const int y = pix / W, xi = pix - y * W;
-    const float x = (float)xi, yf = (float)y;
-    const float d1 = depth_1[(size_t)b * HW + pix];
-    const float2 f = *reinterpret_cast<const float2*>(flow + ((size_t)b * HW + pix) * 2);
-    float sx = 0.f, sy = 0.f, sz = 0.f;
-    const size_t o3 = (size_t)b * 3 * HW + pix, o2 = (size_t)b * 2 * HW + pix, o1 = (size_t)b * HW + pix;
-    if (sf) { sx = sf[o3]; sy = sf[o3 + HW]; sz = sf[o3 + 2 * (size_t)HW]; }
-    Taps tp = make_taps(x + f.x, yf + f.y, H, W);
-    Px o, os;
-    forward_px<false>(ps, d2img, tp, x, yf, d1, sx, sy, sz, o);
-    float a0, a1, a2, b0, b1, b2;
+    const int y = pix / W;
+    const float x = (float)(pix - y * W), yf = (float)y;
+    const size_t o3 = b * 3 * HW + pix, o2 = b * 2 * HW + pix, o1 = b * HW + pix;
+    const PixIn in = load_pixel(depth_1, nullptr, sf, flow, b, HW, pix);
+    const RowTerms rt = row_terms(ps, yf);
+    PixFwd o;
+    pixel_forward(ps, d2img, H, W, x, yf, rt, in, o);
+    float a0, a1, a2, b0v, b1v, b2v;
     // P1: + global_p1, - sf_by_depth ;  wP2: + sf_by_depth, + warped_global_p2
     float gP0, gP1, gP2, gW0, gW1, gW2;
     ld3(G.global_p1, o3, HW, gP0, gP1, gP2);
@@ -632,588 +850,53 @@ __global__ void __launch_bounds__(kThreads) reproject_materialize_bwd_kernel(
     }
     mtv(ps.K, gi0, gi1, gi2, a0, a1, a2);
     gp0 += a0; gp1 += a1; gp2 += a2;
-    mv(ps.R2, gp0, gp1, gp2, b0, b1, b2);        // g_(P1 + sf)
-    if (g_sf) { g_sf[o3] = b0; g_sf[o3 + HW] = b1; g_sf[o3 + 2 * (size_t)HW] = b2; }
-    gP0 += b0; gP1 += b1; gP2 += b2;
+    mv(ps.R2, gp0, gp1, gp2, b0v, b1v, b2v);        // g_(P1 + sf)
+    st3(g_sf, o3, HW, b0v, b1v, b2v);
+    gP0 += b0v; gP1 += b1v; gP2 += b2v;
     if (G.staticflow) {
-      forward_px<false>(ps, d2img, tp, x, yf, d1, 0.f, 0.f, 0.f, os);
+      PixIn in0 = in;
+      in0.sf[0] = in0.sf[1] = in0.sf[2] = 0.f;
+      PixFwd os;
+      pixel_forward(ps, d2img, H, W, x, yf, rt, in0, os);
       if (os.zok) {
         const float gu = G.staticflow[o2], gv = G.staticflow[o2 + HW];
         const float s0 = gu * os.rz, s1 = gv * os.rz, s2 = -(gu * os.i12[0] + gv * os.i12[1]) * os.rz * os.rz;
         mtv(ps.K, s0, s1, s2, a0, a1, a2);
-        mv(ps.R2, a0, a1, a2, b0, b1, b2);
-        gP0 += b0; gP1 += b1; gP2 += b2;
+        mv(ps.R2, a0, a1, a2, b0v, b1v, b2v);
+        gP0 += b0v; gP1 += b1v; gP2 += b2v;
       }
     }
-    // P1 = d1 * (M1 c) + t1
+    // P1 = t1 - d1 * (nM1 c)
     float rx, ry, rz;
-    ray_of(ps.M1, x, yf, rx, ry, rz);
-    if (g_d1) g_d1[o1] = fmaf(gP2, rz, fmaf(gP1, ry, gP0 * rx));
+    ray_of(ps.nM1, x, yf, rx, ry, rz);
+    if (g_d1) g_d1[o1] = -fmaf(gP2, rz, fmaf(gP1, ry, gP0 * rx));
     if (g_d2) {
-      float hu, hv, h1;
+      float hu, hv, h1, gd[4];
       mtv(ps.Kinv, gC0, gC1, gC2, hu, hv, h1);
       if (G.depth_warp) h1 += G.depth_warp[o1];
-      float* gd2img = g_d2 + (size_t)b * HW;
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const float g = tp.w[k] * fmaf(hu, tp.ux[k & 1], fmaf(hv, tp.uy[k >> 1], h1));
-        if (g != 0.f) atomicAdd(gd2img + tp.idx[k], g);
-      }
+      tap_grads(o, hu, hv, h1, gd);
+      scatter4_atomic(g_d2 + b * HW + o.i00, o.sx1, o.sy1, gd);
     }
-  }
-}
-
-// =============================================================================================
-// Pixel-pair path of the fused loss kernels: every matrix-vector product runs on float2 operands (two fp32 lanes per helper
-// call; sm_90 executes each lane as its own fp32 instruction, so the pairing buys fewer index computations and wider loads,
-// not a higher FP32 issue rate).
-//
-// Here each thread owns PAIRS of x-adjacent pixels and every matrix-vector product of the chain runs on float2 operands, the
-// pose entries entering as broadcast scalar operands straight from the constant bank (no shared-memory loads, no
-// register copies). Pose-derived matrices are prepared once per call by pose_prep_kernel and copied into a
-// __constant__ slot with a device-to-device cudaMemcpyToSymbolAsync on the caller's stream (no host round trip).
-struct __align__(16) PoseC {
-  float Kinv[9];   //  0
-  float K[9];      //  9
-  float R2[9];     // 18
-  float nM1[9];    // 27  -(R1 Kinv)                 -(P1 - t1) = d1 * (nM1 c)
-  float A[9];      // 36  R2^T R1 Kinv               p12 = d1 * (A c) + cv + R2^T sf
-  float cv[3];     // 45  R2^T (t1 - t2)
-  float t21[3];    // 48  t2 - t1                    warped_global_p2 - P1 = R2 wpc + t21 + d1 * (nM1 c)
-  float pad[13];
-};
-static_assert(sizeof(PoseC) == 256, "PoseC layout");
-constexpr int kPoseSlots = 3;    // rotating slots: calls in flight on different streams do not share a slot
-constexpr int kPosePairs = 64;   // pairs per launch (larger batches are processed in chunks)
-__constant__ PoseC c_pose[kPoseSlots][kPosePairs];
-__device__ PoseC g_pose_stage[kPoseSlots][kPosePairs];
-
-__global__ void pose_prep_kernel(const float* __restrict__ poses, int B, int slot) {
-  DVD_PDL_ENTER();
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= B) return;
-  const float* p = poses + (size_t)b * DVD_POSE_STRIDE;
-  float Kinv[9], R1[9], R2[9], M1[9], t1[3], t2[3];
-  PoseC& o = g_pose_stage[slot][b];
-  for (int i = 0; i < 9; ++i) {
-    Kinv[i] = p[i]; R1[i] = p[18 + i]; R2[i] = p[27 + i];
-    o.Kinv[i] = Kinv[i]; o.K[i] = p[9 + i]; o.R2[i] = R2[i];
-  }
-  for (int i = 0; i < 3; ++i) { t1[i] = p[36 + i]; t2[i] = p[39 + i]; }
-  mm3(R1, Kinv, M1, false);
-  mm3(R2, M1, o.A, true);
-  for (int i = 0; i < 9; ++i) o.nM1[i] = -M1[i];
-  const float dx = t1[0] - t2[0], dy = t1[1] - t2[1], dz = t1[2] - t2[2];
-  for (int i = 0; i < 3; ++i) {
-    o.cv[i] = fmaf(R2[6 + i], dz, fmaf(R2[3 + i], dy, R2[i] * dx));
-    o.t21[i] = t2[i] - t1[i];
-  }
-}
-
-__device__ __forceinline__ float2 F2(float a) { return make_float2(a, a); }
-// sm_90 has no packed-fp32 instructions: each lane is one round-to-nearest fp32 operation (the same results a packed
-// FFMA2 / FMUL2 / FADD2 gives)
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
-__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
-// a - b as b * -1 + a
-__device__ __forceinline__ float2 sub2(float2 a, float2 b) { return fma2(b, F2(-1.0f), a); }
-// M * v  /  M^T * v  with broadcast matrix entries
-__device__ __forceinline__ void mv2(const float* M, float2 x, float2 y, float2 z, float2& ox, float2& oy, float2& oz) {
-  ox = fma2(F2(M[2]), z, fma2(F2(M[1]), y, mul2(F2(M[0]), x)));
-  oy = fma2(F2(M[5]), z, fma2(F2(M[4]), y, mul2(F2(M[3]), x)));
-  oz = fma2(F2(M[8]), z, fma2(F2(M[7]), y, mul2(F2(M[6]), x)));
-}
-__device__ __forceinline__ void mtv2(const float* M, float2 x, float2 y, float2 z, float2& ox, float2& oy, float2& oz) {
-  ox = fma2(F2(M[6]), z, fma2(F2(M[3]), y, mul2(F2(M[0]), x)));
-  oy = fma2(F2(M[7]), z, fma2(F2(M[4]), y, mul2(F2(M[1]), x)));
-  oz = fma2(F2(M[8]), z, fma2(F2(M[5]), y, mul2(F2(M[2]), x)));
-}
-
-// forward chain of one pixel pair
-struct PairOut {
-  int i00[2], sx1[2], sy1[2];   // nw tap index; element offsets to the ne / sw taps (0 where clamped by the border)
-  float2 w[4];            // bilinear weights; a tap clamped by the border has weight exactly 0
-  float2 x0f, y0f;        // tap origin (the ne / sw / se taps sit at +1 wherever their weight is non-zero)
-  float2 wpc[3], p12[3], i12[3], rz;
-  float2 ex, ey;          // dflow_1_2 - flow_1_2 (zero flow substituted where the projection is rejected)
-  float2 e[3];            // warped_global_p2 - P1 - sf            (kWorld only)
-  bool zok[2];
-};
-
-// Where the four bilinear taps of a pixel come from / where their gradients go.
-struct GlobalTaps {
-  const float* img;   // depth_2 of this pair
-  __device__ __forceinline__ void ld4(int i00, int sx1, int sy1, float (&d)[4]) const {
-    const float* p = img + i00;   // one 64-bit address per pixel, the other taps at small element offsets from it
-    d[0] = __ldg(p); d[1] = __ldg(p + sx1); d[2] = __ldg(p + sy1); d[3] = __ldg(p + sy1 + sx1);
-  }
-};
-__device__ __forceinline__ void red_global_v2(float* p, float a, float b) {
-  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
-}
-__device__ __forceinline__ void red_global_v4(float* p, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-// scatter-add of the four tap gradients of one pixel; the packed kernels require W % 4 == 0, so whenever the nw tap sits
-// on an even column the (nw, ne) and (sw, se) taps are two 8-byte aligned pairs: one vector reduction each
-__device__ __forceinline__ void scatter4_global(float* q, int i00, int sx1, int sy1, const float (&g)[4]) {
-  if (((i00 & 1) == 0) && sx1 == 1) {
-    if (g[0] != 0.f || g[1] != 0.f) red_global_v2(q, g[0], g[1]);
-    if (g[2] != 0.f || g[3] != 0.f) {
-      if (sy1 != 0) red_global_v2(q + sy1, g[2], g[3]);
-      else red_global_v2(q, g[2], g[3]);     // clamped bottom row: both weights are exactly 0 here, kept for form
-    }
-  } else if (((i00 & 3) == 1) && sx1 == 1) {
-    // odd column whose pair still lies inside one 16-byte quad: one 4-wide reduction {0, g, g, 0} per row instead of two
-    // scalar ones (the LSU's reduction rate is per active lane, not per byte: DESIGN.md 8)
-    if (g[0] != 0.f || g[1] != 0.f) red_global_v4(q - 1, 0.f, g[0], g[1], 0.f);
-    if (g[2] != 0.f || g[3] != 0.f) red_global_v4(q - 1 + sy1, 0.f, g[2], g[3], 0.f);
-  } else {
-    if (g[0] != 0.f) atomicAdd(q, g[0]);
-    if (g[1] != 0.f) atomicAdd(q + sx1, g[1]);
-    if (g[2] != 0.f) atomicAdd(q + sy1, g[2]);
-    if (g[3] != 0.f) atomicAdd(q + sy1 + sx1, g[3]);
-  }
-}
-struct GlobalScatter {
-  float* gimg;        // g_depth_2 of this pair (nullptr: no scatter)
-  __device__ __forceinline__ bool on() const { return gimg != nullptr; }
-  __device__ __forceinline__ void add4(int i00, int sx1, int sy1, const float (&g)[4]) const {
-    scatter4_global(gimg + i00, i00, sx1, sy1, g);
-  }
-};
-template <bool kWorld, class Taps>
-__device__ __forceinline__ void pair_forward(const PoseC& ps, const Taps& taps, int H, int W, float2 nx,
-                                             float nyf, float2 fx, float2 fy, float2 d1, float2 sx, float2 sy, float2 sz,
-                                             const float (&rn)[3], const float (&ra)[3], PairOut& o) {
-  const float hw = (float)(W - 1), hh = (float)(H - 1);
-  const float2 nqx = fma2(fx, F2(-1.0f), nx);        // -(x + flow_x)
-  const float2 nqy = fma2(fy, F2(-1.0f), F2(nyf));   // -(y + flow_y)
-  float ixs[2], iys[2], xfs[2], yfs[2];
-  const float nq[2][2] = {{nqx.x, nqy.x}, {nqx.y, nqy.y}};
-#pragma unroll
-  for (int j = 0; j < 2; ++j) {
-    ixs[j] = fminf(hw, fmaxf(-nq[j][0], 0.0f));
-    iys[j] = fminf(hh, fmaxf(-nq[j][1], 0.0f));
-    xfs[j] = floorf(ixs[j]);
-    yfs[j] = floorf(iys[j]);
-    const int xi = (int)xfs[j], yi = (int)yfs[j];
-    o.i00[j] = yi * W + xi;
-    o.sx1[j] = xi < W - 1 ? 1 : 0;
-    o.sy1[j] = yi < H - 1 ? W : 0;
-  }
-  float2 dk[4];
-  {
-    float da[4], db[4];
-    taps.ld4(o.i00[0], o.sx1[0], o.sy1[0], da);
-    taps.ld4(o.i00[1], o.sx1[1], o.sy1[1], db);
-#pragma unroll
-    for (int k = 0; k < 4; ++k) dk[k] = make_float2(da[k], db[k]);
-  }
-  // ---- arithmetic that does not depend on the gathered taps first: it runs while the gather is in flight ----
-  // p12 = d1 (A c) + cv + R2^T sf ; c = (x, y, 1): A c = A[:,0] x + (A[:,1] y + A[:,2]) = -A[:,0] nx + ra
-#pragma unroll
-  for (int k = 0; k < 3; ++k) {
-    const float2 ac = fma2(F2(-ps.A[3 * k]), nx, F2(ra[k]));
-    float2 t = fma2(d1, ac, F2(ps.cv[k]));
-    t = fma2(F2(ps.R2[k]), sx, t);
-    t = fma2(F2(ps.R2[3 + k]), sy, t);
-    o.p12[k] = fma2(F2(ps.R2[6 + k]), sz, t);
-  }
-  mv2(ps.K, o.p12[0], o.p12[1], o.p12[2], o.i12[0], o.i12[1], o.i12[2]);
-  const float2 zz = add2(o.i12[2], F2(1e-8f));
-  o.rz = make_float2(rcp_fast(zz.x), rcp_fast(zz.y));
-  o.zok[0] = !(o.i12[2].x < 1e-3f);
-  o.zok[1] = !(o.i12[2].y < 1e-3f);
-  // dflow - flow = i12.xy * rz - (c.xy + flow)
-  const float2 ex = fma2(o.i12[0], o.rz, nqx), ey = fma2(o.i12[1], o.rz, nqy);
-  o.ex = make_float2(o.zok[0] ? ex.x : -fx.x, o.zok[1] ? ex.y : -fx.y);
-  o.ey = make_float2(o.zok[0] ? ey.x : -fy.x, o.zok[1] ? ey.y : -fy.y);
-  o.x0f = make_float2(xfs[0], xfs[1]);
-  o.y0f = make_float2(yfs[0], yfs[1]);
-  // clamped coordinate == W-1 (H-1) implies a zero fractional part, so the clamped taps need no explicit masking
-  const float2 wx1 = sub2(make_float2(ixs[0], ixs[1]), o.x0f), wy1 = sub2(make_float2(iys[0], iys[1]), o.y0f);
-  const float2 wx0 = fma2(wx1, F2(-1.0f), F2(1.0f)), wy0 = fma2(wy1, F2(-1.0f), F2(1.0f));
-  o.w[0] = mul2(wx0, wy0); o.w[1] = mul2(wx1, wy0); o.w[2] = mul2(wx0, wy1); o.w[3] = mul2(wx1, wy1);
-  float2 et[3];
-  if (kWorld) {
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      const float2 nr = fma2(F2(-ps.nM1[3 * k]), nx, F2(rn[k]));   // -(M1 c)_k
-      et[k] = sub2(fma2(d1, nr, F2(ps.t21[k])), k == 0 ? sx : (k == 1 ? sy : sz));
-    }
-  }
-  // ---- gathered taps ----
-  // wpc = sum_k w_k d2_k Kinv (u_k, v_k, 1) = Kinv (su, sv, s1), u_k = x0f (+1), v_k = y0f (+1)
-  const float2 wd0 = mul2(o.w[0], dk[0]), wd1 = mul2(o.w[1], dk[1]), wd2 = mul2(o.w[2], dk[2]), wd3 = mul2(o.w[3], dk[3]);
-  const float2 eb = add2(wd1, wd3), sb = add2(wd2, wd3);
-  const float2 s1 = add2(add2(wd0, wd1), sb);
-  const float2 su = fma2(o.x0f, s1, eb), sv = fma2(o.y0f, s1, sb);
-  mv2(ps.Kinv, su, sv, s1, o.wpc[0], o.wpc[1], o.wpc[2]);
-  if (kWorld) {
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      float2 t = fma2(F2(ps.R2[3 * k]), o.wpc[0], et[k]);
-      t = fma2(F2(ps.R2[3 * k + 1]), o.wpc[1], t);
-      o.e[k] = fma2(F2(ps.R2[3 * k + 2]), o.wpc[2], t);
-    }
-  }
-}
-
-__device__ __forceinline__ float mask1(const dvd_loss_cfg& c, float m2, float d1, float wz) {
-  return (!c.midas || (d1 < 100.0f && wz < 100.0f)) ? m2 : 0.0f;
-}
-
-// ---------------------------------------------------------------------------------------------
-// Staged variant: the five streamed inputs (28 of the 32 bytes per pixel) travel global -> shared memory as 1-D bulk
-// async copies issued by a producer warp into a ring of STAGES tiles, completion on mbarriers; the 256 consumer threads
-// only see shared-memory latency for them, and the bytes in flight per SM (CTAs x STAGES x 14 KB) no longer depend on
-// occupancy or on how the compiler schedules the loads. Only the bilinear gather of depth_2 is a global load.
-// The bilinear taps of depth_2 are read from global memory and g_depth_2 is accumulated with global reductions; staging
-// either through shared memory is a possible variant that has not been measured on sm_90.
-template <int NP> struct StagedCfg {
-  static constexpr int VEC = 2 * NP;                 // pixels per consumer thread and tile
-  static constexpr int TILE = kThreads * VEC;        // pixels per stage
-  static constexpr int FLOATS = TILE * 7;            // d1, mask, sf.x, sf.y, sf.z, flow (2 floats per pixel)
-};
-
-// stream one tile (pixels [p0, p0 + n) of pair b) into a stage
-template <int TILE>
-__device__ __forceinline__ void produce_tile(float* dst, uint64_t* bar, const float* depth_1, const float* mask_2,
-                                             const float* sf, const float* flow, size_t b, int HW, int p0, int pend) {
-  using namespace tc;
-  const uint32_t n4 = (uint32_t)min(TILE, pend - p0) * 4u;
-  mbar_arrive_expect_tx(bar, n4 * 7u);
-  bulk_g2s(dst, depth_1 + b * HW + p0, n4, bar);
-  bulk_g2s(dst + TILE, mask_2 + b * HW + p0, n4, bar);
-  bulk_g2s(dst + 2 * TILE, sf + (b * 3 + 0) * HW + p0, n4, bar);
-  bulk_g2s(dst + 3 * TILE, sf + (b * 3 + 1) * HW + p0, n4, bar);
-  bulk_g2s(dst + 4 * TILE, sf + (b * 3 + 2) * HW + p0, n4, bar);
-  bulk_g2s(dst + 5 * TILE, flow + (b * HW + p0) * 2, n4 * 2u, bar);
-}
-// a consumer thread's VEC pixels of a stage -> registers
-template <int NP>
-__device__ __forceinline__ void consume_tile(const float* src, int tv, float (&d1)[2 * NP], float (&m2)[2 * NP],
-                                             float (&sx)[2 * NP], float (&sy)[2 * NP], float (&sz)[2 * NP],
-                                             float (&fx)[2 * NP], float (&fy)[2 * NP]) {
-  constexpr int VEC = 2 * NP, TILE = StagedCfg<NP>::TILE;
-  src += tv;
-  if (VEC == 2) {
-    const float2 a = *reinterpret_cast<const float2*>(src), bq = *reinterpret_cast<const float2*>(src + TILE);
-    const float2 c = *reinterpret_cast<const float2*>(src + 2 * TILE), d = *reinterpret_cast<const float2*>(src + 3 * TILE);
-    const float2 e = *reinterpret_cast<const float2*>(src + 4 * TILE);
-    const float4 f = *reinterpret_cast<const float4*>(src + 5 * TILE + tv);
-    d1[0] = a.x; d1[1] = a.y; m2[0] = bq.x; m2[1] = bq.y; sx[0] = c.x; sx[1] = c.y; sy[0] = d.x; sy[1] = d.y;
-    sz[0] = e.x; sz[1] = e.y; fx[0] = f.x; fy[0] = f.y; fx[1] = f.z; fy[1] = f.w;
-  } else {
-    const float4 a = *reinterpret_cast<const float4*>(src), bq = *reinterpret_cast<const float4*>(src + TILE);
-    const float4 c = *reinterpret_cast<const float4*>(src + 2 * TILE), d = *reinterpret_cast<const float4*>(src + 3 * TILE);
-    const float4 e = *reinterpret_cast<const float4*>(src + 4 * TILE);
-    const float4 f = *reinterpret_cast<const float4*>(src + 5 * TILE + tv), g = *reinterpret_cast<const float4*>(src + 5 * TILE + tv + 4);
-    d1[0] = a.x; d1[1] = a.y; d1[2 % VEC] = a.z; d1[3 % VEC] = a.w;
-    m2[0] = bq.x; m2[1] = bq.y; m2[2 % VEC] = bq.z; m2[3 % VEC] = bq.w;
-    sx[0] = c.x; sx[1] = c.y; sx[2 % VEC] = c.z; sx[3 % VEC] = c.w;
-    sy[0] = d.x; sy[1] = d.y; sy[2 % VEC] = d.z; sy[3 % VEC] = d.w;
-    sz[0] = e.x; sz[1] = e.y; sz[2 % VEC] = e.z; sz[3 % VEC] = e.w;
-    fx[0] = f.x; fy[0] = f.y; fx[1] = f.z; fy[1] = f.w; fx[2 % VEC] = g.x; fy[2 % VEC] = g.y; fx[3 % VEC] = g.z; fy[3 % VEC] = g.w;
-  }
-}
-
-// NP pixel pairs per consumer thread, STAGES-deep ring, MINB co-resident CTAs per SM
-template <int NP, int STAGES, int MINB, bool kDry>
-__global__ void __launch_bounds__(kThreads + 32, MINB) reproject_loss_fwd_staged_kernel(
-    const float* __restrict__ depth_1, const float* __restrict__ depth_2, const float* __restrict__ flow,
-    const float* __restrict__ mask_2, const float* __restrict__ sf, dvd_loss_cfg cfg, float* __restrict__ partials,
-    int H, int W, int slot, int b0, int nb, int tiles_per_pair) {
-  DVD_PDL_ENTER();
-  using namespace tc;
-  constexpr int VEC = 2 * NP, TILE = StagedCfg<NP>::TILE, FLOATS = StagedCfg<NP>::FLOATS;
-  extern __shared__ __align__(128) float stage_mem[];
-  __shared__ uint64_t full[STAGES], empty[STAGES];
-  __shared__ float red[kThreads / 32][4];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int HW = H * W, ntiles = nb * tiles_per_pair;
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kThreads / 32); }
-    fence_mbar_init();
-  }
-  __syncthreads();
-  if (warp == kThreads / 32) {
-    // ===== producer =====
-    if (lane == 0) {
-      uint32_t it = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-        const uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
-        mbar_wait(&empty[s], ph ^ 1u);
-        const int bl = tile / tiles_per_pair, t = tile - bl * tiles_per_pair;
-        produce_tile<TILE>(stage_mem + (size_t)s * FLOATS, &full[s], depth_1, mask_2, sf, flow, (size_t)(b0 + bl), HW, t * TILE, HW);
-      }
-    }
-    return;
-  }
-  // ===== consumers =====
-  float2 a_flow = F2(0.f), a_disp = F2(0.f), a_sf = F2(0.f), a_m = F2(0.f);
-  const int tv = threadIdx.x * VEC;
-  uint32_t it = 0;
-  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-    const uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
-    mbar_wait(&full[s], ph);
-    float d1[VEC], m2[VEC], sx[VEC], sy[VEC], sz[VEC], fx[VEC], fy[VEC];
-    consume_tile<NP>(stage_mem + (size_t)s * FLOATS, tv, d1, m2, sx, sy, sz, fx, fy);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[s]);     // values are in registers: hand the stage back
-    const int bl = tile / tiles_per_pair, t = tile - bl * tiles_per_pair;
-    const int p = t * TILE + tv;
-    if (p >= HW) continue;
-    if (kDry) {   // memory-system probe (DVD_REPROJECT_DRY=1): stream the inputs, one gather tap, no chain arithmetic
-      const float g = __ldg(depth_2 + (size_t)(b0 + bl) * HW + p);
-      a_flow = add2(a_flow, make_float2(d1[0] + d1[1] + g, m2[0] + m2[1]));
-      a_sf = add2(a_sf, make_float2(sx[0] + sy[1] + sz[0], fx[0] + fy[1]));
-      if (VEC == 4) a_m = add2(a_m, make_float2(d1[VEC - 1] + m2[VEC - 1] + sx[VEC - 1] + sy[VEC - 2], sz[VEC - 1] + fx[VEC - 1] + fy[VEC - 2]));
-      continue;
-    }
-    const PoseC& ps = c_pose[slot][bl];
-    const float* d2img = depth_2 + (size_t)(b0 + bl) * HW;
-    const int y = p / W, x0 = p - y * W;
-    const float yf = (float)y;
-    float rn[3], ra[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      rn[k] = fmaf(ps.nM1[3 * k + 1], yf, ps.nM1[3 * k + 2]);
-      ra[k] = fmaf(ps.A[3 * k + 1], yf, ps.A[3 * k + 2]);
-    }
-#pragma unroll
-    for (int q = 0; q < NP; ++q) {
-      const int j = 2 * q;
-      const float xf = (float)(x0 + j);
-      const float2 nx = make_float2(-xf, -xf - 1.0f);
-      const float2 dd = make_float2(d1[j], d1[j + 1]);
-      PairOut o;
-      pair_forward<true>(ps, GlobalTaps{d2img}, H, W, nx, -yf, make_float2(fx[j], fx[j + 1]), make_float2(fy[j], fy[j + 1]), dd,
-                         make_float2(sx[j], sx[j + 1]), make_float2(sy[j], sy[j + 1]), make_float2(sz[j], sz[j + 1]), rn, ra, o);
-      const float2 m = make_float2(mask1(cfg, m2[j], dd.x, o.wpc[2].x), mask1(cfg, m2[j + 1], dd.y, o.wpc[2].y));
-      float2 fl, dl, sl;
-      if (cfg.warm) fl = fma2(o.ex, o.ex, mul2(o.ey, o.ey));
-      else fl = make_float2(fabsf(o.ex.x) + fabsf(o.ey.x), fabsf(o.ex.y) + fabsf(o.ey.y));
-      dl = make_float2(disp_term(cfg, o.p12[2].x, o.wpc[2].x), disp_term(cfg, o.p12[2].y, o.wpc[2].y));
-      sl = make_float2(fabsf(o.e[0].x) + fabsf(o.e[1].x) + fabsf(o.e[2].x), fabsf(o.e[0].y) + fabsf(o.e[1].y) + fabsf(o.e[2].y));
-      a_flow = fma2(m, fl, a_flow);
-      a_disp = fma2(m, dl, a_disp);
-      a_sf = fma2(m, sl, a_sf);
-      a_m = add2(a_m, m);
-    }
-  }
-  float s_flow = warp_sum(a_flow.x + a_flow.y), s_disp = warp_sum(a_disp.x + a_disp.y);
-  float s_sf = warp_sum(a_sf.x + a_sf.y), s_m = warp_sum(a_m.x + a_m.y);
-  if (lane == 0) { red[warp][0] = s_flow; red[warp][1] = s_disp; red[warp][2] = s_sf; red[warp][3] = s_m; }
-  asm volatile("bar.sync 1, %0;" ::"n"(kThreads) : "memory");    // consumers only (the producer warp has exited)
-  if (threadIdx.x < 4) {
-    float a = 0.f;
-#pragma unroll
-    for (int w = 0; w < kThreads / 32; ++w) a += red[w][threadIdx.x];
-    partials[(size_t)blockIdx.x * 4 + threadIdx.x] = a;
-  }
-}
-
-// c * sign(v) (0 at v == 0), lane-wise
-__device__ __forceinline__ float2 sgn_scale2(float2 v, float2 c) {
-  const unsigned sx = __float_as_uint(c.x) ^ (__float_as_uint(v.x) & 0x80000000u);   // one LOP3 per lane
-  const unsigned sy = __float_as_uint(c.y) ^ (__float_as_uint(v.y) & 0x80000000u);
-  return make_float2(v.x == 0.f ? 0.f : __uint_as_float(sx), v.y == 0.f ? 0.f : __uint_as_float(sy));
-}
-
-// backward of one pixel pair: returns g_(P1 + sf) and scatters g_depth_2
-template <class Taps, class Scat>
-__device__ __forceinline__ void pair_backward(const PoseC& ps, const dvd_loss_cfg& cfg, const Taps& d2img,
-                                              const Scat& scat, int H, int W, float2 nx, float nyf, float2 fx,
-                                              float2 fy, float2 dd, float2 mm, float2 psx, float2 psy, float2 psz,
-                                              const float (&rn)[3], const float (&ra)[3], float cf, float cd, float2& gv0,
-                                              float2& gv1, float2& gv2) {
-      PairOut o;
-      if (cfg.second_is_disp) pair_forward<false>(ps, d2img, H, W, nx, nyf, fx, fy, dd, psx, psy, psz, rn, ra, o);
-      else                    pair_forward<true>(ps, d2img, H, W, nx, nyf, fx, fy, dd, psx, psy, psz, rn, ra, o);
-      const float2 m = make_float2(mask1(cfg, mm.x, dd.x, o.wpc[2].x), mask1(cfg, mm.y, dd.y, o.wpc[2].y));
-      // --- flow term -> g_i12 (zero where the projection was rejected)
-      const float2 mcf = make_float2(o.zok[0] ? m.x * cf : 0.f, o.zok[1] ? m.y * cf : 0.f);
-      float2 gux, guy;
-      if (cfg.warm) {
-        const float2 t2 = add2(mcf, mcf);
-        gux = mul2(t2, o.ex); guy = mul2(t2, o.ey);
-      } else {
-        gux = sgn_scale2(o.ex, mcf); guy = sgn_scale2(o.ey, mcf);
-      }
-      const float2 gi0 = mul2(gux, o.rz), gi1 = mul2(guy, o.rz);
-      const float2 tt = fma2(gux, o.i12[0], mul2(guy, o.i12[1]));
-      const float2 gi2 = mul2(mul2(tt, o.rz), mul2(o.rz, F2(-1.0f)));
-      float2 gp0, gp1, gp2;   // g_p12 = K^T g_i12
-      mtv2(ps.K, gi0, gi1, gi2, gp0, gp1, gp2);
-      float2 hu, hv, h1;      // Kinv^T g_warped_p2_camera_2
-      float2 ge0 = F2(0.f), ge1 = F2(0.f), ge2 = F2(0.f);
-      const float2 mc = mul2(m, F2(cd));
-      if (cfg.second_is_disp) {
-        const float2 za = o.p12[2], zb = o.wpc[2];
-        float2 gwc2;
-        if (cfg.disp_mode == 0) {
-          const float2 ra2 = make_float2(rcp_fast(fmaxf(za.x, 1e-3f)), rcp_fast(fmaxf(za.y, 1e-3f)));
-          const float2 rb2 = make_float2(rcp_fast(fmaxf(zb.x, 1e-3f)), rcp_fast(fmaxf(zb.y, 1e-3f)));
-          const float2 s = sgn_scale2(sub2(ra2, rb2), mul2(mc, F2(100.0f)));
-          const float2 sa = make_float2(za.x >= 1e-3f ? s.x : 0.f, za.y >= 1e-3f ? s.y : 0.f);
-          const float2 sb = make_float2(zb.x >= 1e-3f ? s.x : 0.f, zb.y >= 1e-3f ? s.y : 0.f);
-          gp2 = fma2(mul2(sa, ra2), mul2(ra2, F2(-1.0f)), gp2);
-          gwc2 = mul2(mul2(sb, rb2), rb2);
-        } else if (cfg.disp_mode == 1) {
-          float g2a[2], g2b[2];
-          const float zas[2] = {za.x, za.y}, zbs[2] = {zb.x, zb.y}, mcs[2] = {mc.x, mc.y};
-#pragma unroll
-          for (int q = 0; q < 2; ++q) {
-            const float a = fmaxf(zas[q], 1e-3f), bb = fmaxf(zbs[q], 1e-3f);
-            const float ra1 = rcp_fast(a), rb1 = rcp_fast(bb);
-            float ga, gb;
-            if (a >= bb) { ga = rb1; gb = -a * rb1 * rb1; }
-            else         { ga = -bb * ra1 * ra1; gb = ra1; }
-            g2a[q] = zas[q] >= 1e-3f ? ga * mcs[q] : 0.f;
-            g2b[q] = zbs[q] >= 1e-3f ? gb * mcs[q] : 0.f;
-          }
-          gp2 = add2(gp2, make_float2(g2a[0], g2a[1]));
-          gwc2 = make_float2(g2b[0], g2b[1]);
-        } else {
-          const float2 s = sgn_scale2(sub2(za, zb), mc);
-          gp2 = add2(gp2, s);
-          gwc2 = mul2(s, F2(-1.0f));
-        }
-        hu = mul2(F2(ps.Kinv[6]), gwc2); hv = mul2(F2(ps.Kinv[7]), gwc2); h1 = mul2(F2(ps.Kinv[8]), gwc2);
-      } else {
-        ge0 = sgn_scale2(o.e[0], mc); ge1 = sgn_scale2(o.e[1], mc); ge2 = sgn_scale2(o.e[2], mc);
-        // warped_global_p2 = R2 wpc + t2  =>  g_wpc = R2^T g_e
-        float2 a0, a1, a2;
-        mtv2(ps.R2, ge0, ge1, ge2, a0, a1, a2);
-        mtv2(ps.Kinv, a0, a1, a2, hu, hv, h1);
-      }
-      // g_(P1 + sf) = R2 g_p12 ; the sf term adds -g_e to both P1 and sf
-      mv2(ps.R2, gp0, gp1, gp2, gv0, gv1, gv2);
-      gv0 = sub2(gv0, ge0); gv1 = sub2(gv1, ge1); gv2 = sub2(gv2, ge2);
-      // scatter to depth_2: g_d2_k = w_k (hu u_k + hv v_k + h1), (u_k, v_k) = (x0f, y0f) (+1)
-      if (scat.on()) {
-        const float2 base = fma2(hu, o.x0f, fma2(hv, o.y0f, h1));
-        const float2 bx = add2(base, hu);
-        const float2 g0 = mul2(o.w[0], base), g1 = mul2(o.w[1], bx);
-        const float2 g2 = mul2(o.w[2], add2(base, hv)), g3 = mul2(o.w[3], add2(bx, hv));
-        const float ga[4] = {g0.x, g1.x, g2.x, g3.x}, gb[4] = {g0.y, g1.y, g2.y, g3.y};
-        scat.add4(o.i00[0], o.sx1[0], o.sy1[0], ga);
-        scat.add4(o.i00[1], o.sx1[1], o.sy1[1], gb);
-      }
-}
-
-// staged backward (same producer / consumer ring as the staged forward), NP pixel pairs per consumer thread
-template <int NP, int STAGES, int MINB>
-__global__ void __launch_bounds__(kThreads + 32, MINB) reproject_loss_bwd_staged_kernel(
-    const float* __restrict__ depth_1, const float* __restrict__ depth_2, const float* __restrict__ flow,
-    const float* __restrict__ mask_2, const float* __restrict__ sf, dvd_loss_cfg cfg, const float* __restrict__ scalars,
-    float gscale, const float* __restrict__ gscale_dev, float* __restrict__ g_sf, float* __restrict__ g_d2, int H, int W,
-    int slot, int b0, int nb, int tiles_per_pair) {
-  DVD_PDL_ENTER();
-  using namespace tc;
-  constexpr int VEC = 2 * NP, TILE = StagedCfg<NP>::TILE, FLOATS = StagedCfg<NP>::FLOATS;
-  extern __shared__ __align__(128) float stage_mem[];
-  __shared__ uint64_t full[STAGES], empty[STAGES];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int HW = H * W, ntiles = nb * tiles_per_pair;
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kThreads / 32); }
-    fence_mbar_init();
-  }
-  __syncthreads();
-  if (warp == kThreads / 32) {
-    if (lane == 0) {
-      uint32_t it = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-        const uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
-        mbar_wait(&empty[s], ph ^ 1u);
-        const int bl = tile / tiles_per_pair, t = tile - bl * tiles_per_pair;
-        produce_tile<TILE>(stage_mem + (size_t)s * FLOATS, &full[s], depth_1, mask_2, sf, flow, (size_t)(b0 + bl), HW, t * TILE, HW);
-      }
-    }
-    return;
-  }
-  const float gs = gscale * (gscale_dev ? __ldg(gscale_dev) : 1.0f);
-  const float cf = __ldg(scalars + DVD_S_CF) * gs;
-  const float cd = __ldg(scalars + DVD_S_CD) * gs;
-  const int tv = threadIdx.x * VEC;
-  uint32_t it = 0;
-  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-    const uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
-    mbar_wait(&full[s], ph);
-    float d1[VEC], m2[VEC], sx[VEC], sy[VEC], sz[VEC], fx[VEC], fy[VEC], ox[VEC], oy[VEC], oz[VEC];
-    consume_tile<NP>(stage_mem + (size_t)s * FLOATS, tv, d1, m2, sx, sy, sz, fx, fy);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[s]);
-    const int bl = tile / tiles_per_pair, t = tile - bl * tiles_per_pair;
-    const int p = t * TILE + tv;
-    if (p >= HW) continue;
-    const PoseC& ps = c_pose[slot][bl];
-    const size_t b = (size_t)(b0 + bl);
-    const float* d2img = depth_2 + b * HW;
-    float* gd2img = g_d2 ? g_d2 + b * HW : nullptr;
-    const int y = p / W, x0 = p - y * W;
-    const float yf = (float)y;
-    float rn[3], ra[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      rn[k] = fmaf(ps.nM1[3 * k + 1], yf, ps.nM1[3 * k + 2]);
-      ra[k] = fmaf(ps.A[3 * k + 1], yf, ps.A[3 * k + 2]);
-    }
-#pragma unroll
-    for (int q = 0; q < NP; ++q) {
-      const int j = 2 * q;
-      const float xf = (float)(x0 + j);
-      const float2 nx = make_float2(-xf, -xf - 1.0f);
-      float2 gv0, gv1, gv2;
-      pair_backward(ps, cfg, GlobalTaps{d2img}, GlobalScatter{gd2img}, H, W, nx, -yf, make_float2(fx[j], fx[j + 1]), make_float2(fy[j], fy[j + 1]),
-                    make_float2(d1[j], d1[j + 1]), make_float2(m2[j], m2[j + 1]), make_float2(sx[j], sx[j + 1]),
-                    make_float2(sy[j], sy[j + 1]), make_float2(sz[j], sz[j + 1]), rn, ra, cf, cd, gv0, gv1, gv2);
-      ox[j] = gv0.x; ox[j + 1] = gv0.y; oy[j] = gv1.x; oy[j + 1] = gv1.y; oz[j] = gv2.x; oz[j + 1] = gv2.y;
-    }
-    float* gsp = g_sf + b * 3 * HW + p;
-    store_vec<VEC>(gsp, ox);
-    store_vec<VEC>(gsp + HW, oy);
-    store_vec<VEC>(gsp + 2 * (size_t)HW, oz);
   }
 }
 
 // ---------------------------------------------------------------------------------------------
-static int pick_vec(int B, int H, int W, std::initializer_list<const void*> ptrs, int max_vec = 4) {
+static int pick_vec(int B, int H, int W, std::initializer_list<const void*> ptrs) {
   bool al = true;
   for (const void* p : ptrs) al = al && (p == nullptr || aligned16(p));
   long total = (long)B * H * W;
-#ifdef DVD_PROFILING
-  if (const char* ev = getenv("DVD_REPROJECT_VEC")) {   // tuning override: 1, 2 or 4
-    int v = atoi(ev);
-    if ((v == 4 && al && W % 4 == 0) || (v == 2 && al && W % 2 == 0)) return v;
-    if (v == 1) return 1;
-  }
-#endif
   // wide vectors only when enough threads remain to cover HBM latency (>= 512 / 256 threads per SM)
-  if (max_vec >= 4 && al && W % 4 == 0 && total / 4 >= (long)num_sms() * 512) return 4;
-  if (max_vec >= 2 && al && W % 2 == 0 && total / 2 >= (long)num_sms() * 256) return 2;
+  if (al && W % 4 == 0 && total / 4 >= (long)num_sms() * 512) return 4;
+  if (al && W % 2 == 0 && total / 2 >= (long)num_sms() * 256) return 2;
   return 1;
 }
 
 // ~8 CTAs of 256 threads per SM over the whole grid, split evenly over the pairs: a mild over-subscription lets short CTAs
-// retire and refill continuously instead of finishing together.
-template <typename K>
-static dim3 grid_for(K, int B, int items_per_pair) {
+// retire and refill continuously instead of finishing together. 8 CTAs per SM is also the hardware maximum for 256
+// threads, so this bounds the partial-sum scratch of the generic forward.
+static dim3 grid_for(int B, int items_per_pair) {
   int per_pair = (items_per_pair + kThreads - 1) / kThreads;
-  int cap = (num_sms() * 8 + B - 1) / B;
-  if (cap < 1) cap = 1;
-  if (per_pair > cap) per_pair = cap;
-  if (per_pair < 1) per_pair = 1;
-  return dim3((unsigned)per_pair, (unsigned)B, 1);
-}
-// upper bound used to size the partial-sum scratch (8 CTAs per SM is the hardware maximum for 256 threads)
-static dim3 grid_bound(int B, int items_per_pair) {
-  int per_pair = (items_per_pair + kThreads - 1) / kThreads;
-  int cap = (num_sms() * 8 + B - 1) / B;
+  const int cap = (num_sms() * 8 + B - 1) / B;
   if (per_pair > cap) per_pair = cap;
   if (per_pair < 1) per_pair = 1;
   return dim3((unsigned)per_pair, (unsigned)B, 1);
@@ -1278,6 +961,25 @@ static int release_pose_slot(int slot, cudaStream_t st) {
   return 0;
 }
 
+// Walks the pairs in chunks of at most kPosePairs: stages a chunk's poses, calls launch(slot, b0, nb) to enqueue the
+// kernel that reads them, then releases the slot.
+template <class Launch>
+static int for_pose_chunks(const float* poses, int B, cudaStream_t st, Launch&& launch) {
+  for (int b0 = 0; b0 < B; b0 += kPosePairs) {
+    const int nb = std::min(B - b0, kPosePairs);
+    int slot = 0;
+    if (int e = stage_poses(poses, b0, nb, st, &slot)) return e;
+    if (int e = launch(slot, b0, nb)) return e;
+    if (int e = release_pose_slot(slot, st)) return e;
+  }
+  return 0;
+}
+
+// partial-sum quads written by the staged forward for one chunk of nb pairs
+static int staged_quads(int nb, int HW) { return std::min(nb * ((HW + kTile - 1) / kTile), kFwdCtasPerSm * num_sms()); }
+// grid of the generic forward (N = 2 pixels per thread when W is even)
+static dim3 generic_fwd_grid(int B, int H, int W) { return grid_for(B, W % 2 == 0 ? H * W / 2 : H * W); }
+
 static int check_shape(int B, int H, int W) {
   DVD_ARG_CHECK(B >= 1 && H >= 2 && W >= 2, "bad shape B=%d H=%d W=%d (need B>=1, H,W>=2)", B, H, W);
   DVD_ARG_CHECK(B <= 65535, "B=%d exceeds gridDim.y", B);
@@ -1291,13 +993,10 @@ using namespace dvd;
 
 extern "C" int dvd_reproject_partials_size(int B, int H, int W) {
   if (B < 1 || H < 1 || W < 1) return 0;
-  // upper bound over every VEC choice
-  dim3 g = grid_bound(B, H * W);
-  long quads = (long)g.x * g.y;
-  // staged forward: one quad per persistent CTA, per chunk of kPosePairs pairs
-  const long staged = (long)((B + kPosePairs - 1) / kPosePairs) * 3 * num_sms();
-  if (staged > quads) quads = staged;
-  return (int)(quads * 4);
+  long staged = 0;
+  for (int b0 = 0; b0 < B; b0 += kPosePairs) staged += staged_quads(std::min(B - b0, kPosePairs), H * W);
+  const dim3 g = generic_fwd_grid(B, H, W);
+  return (int)(std::max(staged, (long)g.x * g.y) * 4);
 }
 
 extern "C" int dvd_unproject_fwd(const float* depth, const float* poses, float* P, int B, int H, int W, int which,
@@ -1307,10 +1006,10 @@ extern "C" int dvd_unproject_fwd(const float* depth, const float* poses, float* 
   DVD_ARG_CHECK(which == 1 || which == 2, "which must be 1 or 2");
   cudaStream_t st = (cudaStream_t)stream;
   int vec = pick_vec(B, H, W, {depth, P});
-  const int ipp = H * W / vec;
-  if (vec == 4) dvd::launch(unproject_fwd_kernel<4>, grid_for(unproject_fwd_kernel<4>, B, ipp), kThreads, 0, st, depth, poses, P, H, W, which);
-  else if (vec == 2) dvd::launch(unproject_fwd_kernel<2>, grid_for(unproject_fwd_kernel<2>, B, ipp), kThreads, 0, st, depth, poses, P, H, W, which);
-  else dvd::launch(unproject_fwd_kernel<1>, grid_for(unproject_fwd_kernel<1>, B, ipp), kThreads, 0, st, depth, poses, P, H, W, which);
+  const dim3 g = grid_for(B, H * W / vec);
+  if (vec == 4) dvd::launch(unproject_fwd_kernel<4>, g, kThreads, 0, st, depth, poses, P, H, W, which);
+  else if (vec == 2) dvd::launch(unproject_fwd_kernel<2>, g, kThreads, 0, st, depth, poses, P, H, W, which);
+  else dvd::launch(unproject_fwd_kernel<1>, g, kThreads, 0, st, depth, poses, P, H, W, which);
   DVD_CUDA_LAUNCH_CHECK("unproject_fwd");
   return 0;
 }
@@ -1322,10 +1021,10 @@ extern "C" int dvd_unproject_bwd(const float* gP, const float* poses, float* gde
   DVD_ARG_CHECK(which == 1 || which == 2, "which must be 1 or 2");
   cudaStream_t st = (cudaStream_t)stream;
   int vec = pick_vec(B, H, W, {gP, gdepth});
-  const int ipp = H * W / vec;
-  if (vec == 4) dvd::launch(unproject_bwd_kernel<4>, grid_for(unproject_bwd_kernel<4>, B, ipp), kThreads, 0, st, gP, poses, gdepth, H, W, which);
-  else if (vec == 2) dvd::launch(unproject_bwd_kernel<2>, grid_for(unproject_bwd_kernel<2>, B, ipp), kThreads, 0, st, gP, poses, gdepth, H, W, which);
-  else dvd::launch(unproject_bwd_kernel<1>, grid_for(unproject_bwd_kernel<1>, B, ipp), kThreads, 0, st, gP, poses, gdepth, H, W, which);
+  const dim3 g = grid_for(B, H * W / vec);
+  if (vec == 4) dvd::launch(unproject_bwd_kernel<4>, g, kThreads, 0, st, gP, poses, gdepth, H, W, which);
+  else if (vec == 2) dvd::launch(unproject_bwd_kernel<2>, g, kThreads, 0, st, gP, poses, gdepth, H, W, which);
+  else dvd::launch(unproject_bwd_kernel<1>, g, kThreads, 0, st, gP, poses, gdepth, H, W, which);
   DVD_CUDA_LAUNCH_CHECK("unproject_bwd");
   return 0;
 }
@@ -1359,54 +1058,35 @@ extern "C" int dvd_reproject_loss_fwd(const float* depth_1, const float* depth_2
   DVD_ARG_CHECK(depth_1 && depth_2 && flow_1_2 && mask_2 && sf && poses && partials && scalars, "null pointer");
   DVD_ARG_CHECK(aligned16(partials), "partials must be 16-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
-  int vec = pick_vec(B, H, W, {depth_1, mask_2, sf, flow_1_2});
-  const int ipp = H * W / vec;
-  dim3 g;
-  // DVD_REPROJECT_SCALAR=1 forces the generic scalar kernels (any shape); DVD_REPROJECT_DRY=1 is a memory-system probe
-  // DVD_REPROJECT_SCALAR=1 (any build) forces the generic scalar kernels - a cross-check with identical results; the
-  // arithmetic-free memory probe exists in -DDVD_PROFILING builds only
-  static const bool packed = !(getenv("DVD_REPROJECT_SCALAR") && atoi(getenv("DVD_REPROJECT_SCALAR")));
-#ifdef DVD_PROFILING
-  static const bool dry = getenv("DVD_REPROJECT_DRY") && atoi(getenv("DVD_REPROJECT_DRY"));
-#else
-  constexpr bool dry = false;
-#endif
-  if (vec == 4 && packed) {
-    // packed-FP32 kernel, bulk-async staged inputs: 1 pixel pair per consumer thread, 4-deep ring, 3 CTAs per SM
-    //
-    const void* fn = dry ? (const void*)reproject_loss_fwd_staged_kernel<1, 4, 3, true>
-                         : (const void*)reproject_loss_fwd_staged_kernel<1, 4, 3, false>;
-    constexpr int np = 1, stages = 4, ctas = 3;
-    const int tile = kThreads * 2 * np, smem = stages * tile * 7 * 4;
-    if (int e = set_smem_once(fn, smem)) return e;
-    const int tiles_per_pair = (H * W + tile - 1) / tile;
-    unsigned nq = 0;
-    for (int b0 = 0; b0 < B; b0 += kPosePairs) {
-      int nb = B - b0 < kPosePairs ? B - b0 : kPosePairs;
-      int slot = 0;
-      if (int e = stage_poses(poses, b0, nb, st, &slot)) return e;
-      int gx = nb * tiles_per_pair;
-      if (gx > ctas * num_sms()) gx = ctas * num_sms();
-      float* part = partials + (size_t)nq * 4;
-      int b0v = b0, tpp = tiles_per_pair, Hh = H, Ww = W;
-      dvd_loss_cfg cfgv = *cfg;
-      void* args[] = {(void*)&depth_1, (void*)&depth_2, (void*)&flow_1_2, (void*)&mask_2, (void*)&sf, (void*)&cfgv, (void*)&part,
-                      (void*)&Hh, (void*)&Ww, (void*)&slot, (void*)&b0v, (void*)&nb, (void*)&tpp};
-      DVD_CUDA_CALL(cudaLaunchKernel(fn, dim3((unsigned)gx), dim3(kThreads + 32), args, (size_t)smem, st));
-      if (int e = release_pose_slot(slot, st)) return e;
-      nq += (unsigned)gx;
-    }
-    g = dim3(nq, 1, 1);
+  const int HW = H * W;
+  // staged: 16-byte bulk copies need W % 4 == 0 and aligned bases; below the size threshold the generic kernel is faster
+  const bool staged = pick_vec(B, H, W, {depth_1, mask_2, sf, flow_1_2}) == 4;
+  if (staged)
+    if (int e = set_smem_once((const void*)reproject_loss_fwd_staged_kernel, kStagedSmem)) return e;
+  int nq = 0;
+  if (staged) {
+    int e = for_pose_chunks(poses, B, st, [&](int slot, int b0, int nb) -> int {
+      const int gx = staged_quads(nb, HW);
+      reproject_loss_fwd_staged_kernel<<<gx, kThreads + 32, kStagedSmem, st>>>(
+          depth_1, depth_2, flow_1_2, mask_2, sf, *cfg, partials + (size_t)nq * 4, H, W, slot, b0, nb,
+          (HW + kTile - 1) / kTile);
+      nq += gx;
+      DVD_CUDA_LAUNCH_CHECK("reproject_loss_fwd");
+      return 0;
+    });
+    if (e) return e;
   } else {
-    if (vec == 4) g = grid_for(reproject_loss_fwd_kernel<4, 3>, B, ipp);
-    else if (vec == 2) g = grid_for(reproject_loss_fwd_kernel<2, 4>, B, ipp);
-    else g = grid_for(reproject_loss_fwd_kernel<1, 4>, B, ipp);
-    if (vec == 4) dvd::launch(reproject_loss_fwd_kernel<4, 3>, g, kThreads, 0, st, depth_1, depth_2, flow_1_2, mask_2, sf, poses, *cfg, partials, H, W);
-    else if (vec == 2) dvd::launch(reproject_loss_fwd_kernel<2, 4>, g, kThreads, 0, st, depth_1, depth_2, flow_1_2, mask_2, sf, poses, *cfg, partials, H, W);
-    else dvd::launch(reproject_loss_fwd_kernel<1, 4>, g, kThreads, 0, st, depth_1, depth_2, flow_1_2, mask_2, sf, poses, *cfg, partials, H, W);
+    const dim3 g = generic_fwd_grid(B, H, W);
+    if (W % 2 == 0)
+      dvd::launch(reproject_loss_fwd_kernel<2>, g, kThreads, 0, st, depth_1, depth_2, flow_1_2, mask_2, sf, *cfg, partials,
+                  H, W, poses);
+    else
+      dvd::launch(reproject_loss_fwd_kernel<1>, g, kThreads, 0, st, depth_1, depth_2, flow_1_2, mask_2, sf, *cfg, partials,
+                  H, W, poses);
+    DVD_CUDA_LAUNCH_CHECK("reproject_loss_fwd");
+    nq = (int)(g.x * g.y);
   }
-  DVD_CUDA_LAUNCH_CHECK("reproject_loss_fwd");
-  dvd::launch(reproject_finalize_kernel, 1, 256, 0, st, partials, (int)(g.x * g.y), *cfg, scalars);
+  dvd::launch(reproject_finalize_kernel, 1, 256, 0, st, partials, nq, *cfg, scalars);
   DVD_CUDA_LAUNCH_CHECK("reproject_finalize");
   return 0;
 }
@@ -1419,43 +1099,25 @@ extern "C" int dvd_reproject_loss_bwd(const float* depth_1, const float* depth_2
   if (int e = check_cfg(cfg)) return e;
   DVD_ARG_CHECK(depth_1 && depth_2 && flow_1_2 && mask_2 && sf && poses && scalars && g_sf, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  if (g_depth_2) DVD_CUDA_CALL(cudaMemsetAsync(g_depth_2, 0, (size_t)B * H * W * sizeof(float), st));
-#ifdef DVD_PROFILING
-  if (getenv("DVD_REPROJECT_BWD_NOSCATTER")) g_depth_2 = nullptr;   // profiling probe only: skip the scatter-add
-#endif
-  // the scatter-add backward runs one pixel per thread: more warps in flight hide the red.global latency
-  static const bool packed = !(getenv("DVD_REPROJECT_SCALAR") && atoi(getenv("DVD_REPROJECT_SCALAR")));
-  const int vecp = pick_vec(B, H, W, {depth_1, mask_2, sf, flow_1_2, g_sf}, 4);
-  if (packed && vecp == 4) {
-    // packed-FP32 kernel, bulk-async staged inputs: 1 pixel pair per consumer thread, 4-deep ring, 2 CTAs per SM
-    const void* fn = (const void*)reproject_loss_bwd_staged_kernel<1, 4, 2>;
-    constexpr int np = 1, stages = 4, ctas = 2;
-    const int tile = kThreads * 2 * np, smem = stages * tile * 7 * 4;
-    if (int e = set_smem_once(fn, smem)) return e;
-    const int tiles_per_pair = (H * W + tile - 1) / tile;
-    for (int b0 = 0; b0 < B; b0 += kPosePairs) {
-      int nb = B - b0 < kPosePairs ? B - b0 : kPosePairs;
-      int slot = 0;
-      if (int e = stage_poses(poses, b0, nb, st, &slot)) return e;
-      int gx = nb * tiles_per_pair;
-      if (gx > ctas * num_sms()) gx = ctas * num_sms();
-      int b0v = b0, tpp = tiles_per_pair, Hh = H, Ww = W;
-      dvd_loss_cfg cfgv = *cfg;
-      void* args[] = {(void*)&depth_1, (void*)&depth_2, (void*)&flow_1_2, (void*)&mask_2, (void*)&sf, (void*)&cfgv, (void*)&scalars,
-                      (void*)&gscale, (void*)&gscale_dev, (void*)&g_sf, (void*)&g_depth_2, (void*)&Hh, (void*)&Ww, (void*)&slot,
-                      (void*)&b0v, (void*)&nb, (void*)&tpp};
-      DVD_CUDA_CALL(cudaLaunchKernel(fn, dim3((unsigned)gx), dim3(kThreads + 32), args, (size_t)smem, st));
-      if (int e = release_pose_slot(slot, st)) return e;
-    }
-    return 0;
-  }
-  int vec = pick_vec(B, H, W, {depth_1, mask_2, sf, flow_1_2, g_sf}, 1);
-  const int ipp = H * W / vec;
-  dim3 g = vec == 4 ? grid_for(reproject_loss_bwd_kernel<4>, B, ipp)
-                    : (vec == 2 ? grid_for(reproject_loss_bwd_kernel<2>, B, ipp) : grid_for(reproject_loss_bwd_kernel<1>, B, ipp));
-  if (vec == 4) dvd::launch(reproject_loss_bwd_kernel<4>, g, kThreads, 0, st, depth_1, depth_2, flow_1_2, mask_2, sf, poses, *cfg, scalars, gscale, gscale_dev, g_sf, g_depth_2, H, W);
-  else if (vec == 2) dvd::launch(reproject_loss_bwd_kernel<2>, g, kThreads, 0, st, depth_1, depth_2, flow_1_2, mask_2, sf, poses, *cfg, scalars, gscale, gscale_dev, g_sf, g_depth_2, H, W);
-  else dvd::launch(reproject_loss_bwd_kernel<1>, g, kThreads, 0, st, depth_1, depth_2, flow_1_2, mask_2, sf, poses, *cfg, scalars, gscale, gscale_dev, g_sf, g_depth_2, H, W);
+  const int HW = H * W;
+  if (g_depth_2) DVD_CUDA_CALL(cudaMemsetAsync(g_depth_2, 0, (size_t)B * HW * sizeof(float), st));
+  // staged: bulk copies and vector reductions need W % 4 == 0 and aligned bases; below the size threshold the generic
+  // kernel is faster
+  const bool staged = pick_vec(B, H, W, {depth_1, mask_2, sf, flow_1_2, g_sf, g_depth_2}) == 4;
+  if (staged)
+    if (int e = set_smem_once((const void*)reproject_loss_bwd_staged_kernel, kStagedSmem)) return e;
+  if (staged)
+    return for_pose_chunks(poses, B, st, [&](int slot, int b0, int nb) -> int {
+      const int tiles_per_pair = (HW + kTile - 1) / kTile;
+      const int gx = std::min(nb * tiles_per_pair, kBwdCtasPerSm * num_sms());
+      reproject_loss_bwd_staged_kernel<<<gx, kThreads + 32, kStagedSmem, st>>>(
+          depth_1, depth_2, flow_1_2, mask_2, sf, *cfg, scalars, gscale, gscale_dev, g_sf, g_depth_2, H, W, slot, b0, nb,
+          tiles_per_pair);
+      DVD_CUDA_LAUNCH_CHECK("reproject_loss_bwd");
+      return 0;
+    });
+  dvd::launch(reproject_loss_bwd_kernel, grid_for(B, HW), kThreads, 0, st, depth_1, depth_2, flow_1_2, mask_2, sf, *cfg,
+              scalars, gscale, gscale_dev, g_sf, g_depth_2, H, W, poses);
   DVD_CUDA_LAUNCH_CHECK("reproject_loss_bwd");
   return 0;
 }
@@ -1468,10 +1130,9 @@ extern "C" int dvd_reproject_materialize(const float* depth_1, const float* dept
   if (int e = check_shape(B, H, W)) return e;
   DVD_ARG_CHECK(depth_1 && depth_2 && flow_1_2 && poses, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  dim3 g = grid_for(reproject_materialize_kernel, B, H * W);
-  dvd::launch(reproject_materialize_kernel, g, kThreads, 0, st, depth_1, depth_2, flow_1_2, sf, poses, global_p1, sf_by_depth,
-                                                       warped_global_p2, warped_p2_camera_2, p1_camera_2, dflow_1_2,
-                                                       staticflow_1_2, depth_image_1_2, depth_warp_1_2, H, W);
+  dvd::launch(reproject_materialize_kernel, grid_for(B, H * W), kThreads, 0, st, depth_1, depth_2, flow_1_2, sf, global_p1,
+              sf_by_depth, warped_global_p2, warped_p2_camera_2, p1_camera_2, dflow_1_2, staticflow_1_2, depth_image_1_2,
+              depth_warp_1_2, H, W, poses);
   DVD_CUDA_LAUNCH_CHECK("reproject_materialize");
   return 0;
 }
@@ -1488,11 +1149,10 @@ extern "C" int dvd_reproject_materialize_bwd(const float* depth_1, const float* 
   DVD_ARG_CHECK(depth_1 && depth_2 && flow_1_2 && poses, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   if (g_depth_2) DVD_CUDA_CALL(cudaMemsetAsync(g_depth_2, 0, (size_t)B * H * W * sizeof(float), st));
-  MatGrads G{g_global_p1, g_sf_by_depth, g_warped_global_p2, g_warped_p2_camera_2, g_p1_camera_2,
-             g_dflow_1_2, g_staticflow_1_2, g_depth_image_1_2, g_depth_warp_1_2};
-  dim3 g = grid_for(reproject_materialize_bwd_kernel, B, H * W);
-  dvd::launch(reproject_materialize_bwd_kernel, g, kThreads, 0, st, depth_1, depth_2, flow_1_2, sf, poses, G, g_depth_1, g_depth_2,
-                                                         g_sf, H, W);
+  const MatGrads G{g_global_p1, g_sf_by_depth, g_warped_global_p2, g_warped_p2_camera_2, g_p1_camera_2,
+                   g_dflow_1_2, g_staticflow_1_2, g_depth_image_1_2, g_depth_warp_1_2};
+  dvd::launch(reproject_materialize_bwd_kernel, grid_for(B, H * W), kThreads, 0, st, depth_1, depth_2, flow_1_2, sf, G,
+              g_depth_1, g_depth_2, g_sf, H, W, poses);
   DVD_CUDA_LAUNCH_CHECK("reproject_materialize_bwd");
   return 0;
 }

@@ -77,9 +77,10 @@ def test_fused_loss_and_grads_match_reference_fixture(reproject_golden, mode):
     assert rel_err(d1.grad, m['g_d1']) < 1e-4
 
 
-@pytest.mark.parametrize('shape', [(1, 32, 48), (3, 30, 50), (2, 17, 23), (5, 64, 96)])
+@pytest.mark.parametrize('shape', [(1, 32, 48), (3, 30, 50), (2, 17, 23), (5, 64, 96), (65, 6, 10), (65, 96, 128)])
 def test_fused_matches_oracle_on_seeded_inputs(shape):
-    """Odd sizes exercise the VEC=1/2 paths; (5,64,96) the wider path."""
+    """Odd and small shapes run the generic kernels, (65, 96, 128) the staged ones (the size condition holds up to
+    390 SMs); B = 65 crosses the 64-pair chunk of constant-bank poses of the staged path."""
     from dvd_b200 import ops, synthetic
     from oracle import geometry
     B, H, W = shape
@@ -110,10 +111,11 @@ def test_fused_matches_oracle_on_seeded_inputs(shape):
 
 @pytest.mark.parametrize('case', [(4, 224, 384, 3.0, 'joint_disp'), (4, 224, 384, 14.0, 'joint_sf'),
                                   (5, 203, 384, 9.0, 'warm_disp'), (4, 224, 384, 40.0, 'joint_ratio_nomidas')])
-def test_packed_staged_path_matches_oracle(case):
-    """Shapes large enough for the packed-FP32 kernels (FFMA2 math, constant-bank poses, bulk-async staged inputs,
-    8-byte vector reductions for the scatter). Small and very large flows (border clamps), H = 203 leaves a ragged
-    last tile; every loss mode of the reference is covered (smf.py:285-324,140-150)."""
+def test_staged_path_matches_oracle(case):
+    """The staged kernels (bulk-async staged inputs, vector reductions for the scatter) against the oracle. Small and
+    very large flows (border clamps), H = 203 leaves a ragged last tile; every loss mode of the reference is covered
+    (smf.py:285-324,140-150). The same inputs through the generic kernels (16-byte misaligned copies) give a bitwise
+    equal g_sf: both paths run the same per-pixel functions."""
     from dvd_b200 import ops, synthetic
     from oracle import geometry
     B, H, W, sigma, mode = case
@@ -140,6 +142,23 @@ def test_packed_staged_path_matches_oracle(case):
     loss.backward()
     for mine, ref, name in ((d1g.grad, go[0], 'g_d1'), (d2g.grad, go[1], 'g_d2'), (sfg.grad, go[2], 'g_sf')):
         assert rel_err(mine, ref) < 2e-4, name
+
+    def misaligned(t):   # contiguous copy whose data pointer sits 4 bytes past a 16-byte boundary
+        buf = torch.empty(t.numel() + 4, dtype=t.dtype, device=t.device)
+        out = buf[1:1 + t.numel()].view(t.shape)
+        out.copy_(t)
+        return out
+
+    cfg = _cfg(kw)
+    ins = (d1g.detach(), d2g.detach(), b['flow_1_2'], mask, sfg.detach(), poses)
+    s_st = ops.reproject_loss_fwd(*ins, cfg)
+    g_st, gd_st = ops.reproject_loss_bwd(*ins, cfg, s_st)
+    mis = [misaligned(t) for t in ins[:5]] + [poses]
+    s_gen = ops.reproject_loss_fwd(*mis, cfg)
+    g_gen, gd_gen = ops.reproject_loss_bwd(*mis, cfg, s_st)
+    assert torch.equal(g_gen, g_st)
+    assert abs(s_gen[3].item() - s_st[3].item()) <= 1e-6 * abs(s_st[3].item())
+    assert rel_err(gd_gen, gd_st) < 1e-6
 
 
 def test_border_and_empty_mask_edge_cases():
