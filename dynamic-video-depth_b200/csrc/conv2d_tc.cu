@@ -8,7 +8,8 @@
 //   grouped 3x3 (32 groups)      torchvision Bottleneck.conv2 (ResNeXt), as block-diagonal 64-channel GEMM blocks
 //   the data gradient of each    same kernel: transposed (BatchNorm-scaled) weight image, a tap table instead of a fixed
 //                                3x3 stencil, stride-2 gradients as 4 sub-pixel phases with a strided store
-//   the weight gradient of each  conv_wgrad_kernel below (K = pixels, both operands channel-contiguous)
+//   the weight gradient of each  conv_wgrad_kernel below (K = pixels, both operands channel-contiguous: one from registers,
+//                                the other transposed in shared memory)
 // with the elementwise neighbours folded into the epilogue:  y = round_tf32(mask * relu(acc * scale + shift + res + res2))
 // (eval-mode BatchNorm / bias, residual adds, ReLU forward; residual-gradient add and ReLU mask backward).
 //
@@ -25,6 +26,7 @@
 
 #include <cuda.h>
 #include <cudaTypedefs.h>
+#include <type_traits>
 
 namespace dvd {
 namespace {
@@ -413,22 +415,33 @@ __global__ void __launch_bounds__(256) conv_pack_batch_kernel(const dvd_pack_ite
 // =====================================================================================================================
 // Weight gradient:  D[m][n] += sum over pixels  Mop[px (+off), m] * Nop[px (+off), n]
 // normally Mop = gy (out-channels), Nop = x shifted by the tap and sampled with the convolution stride; `swap` exchanges
-// the roles (needs 128 | M-channels). GEMM with K = pixels. Both operands arrive channel-contiguous (MN-major) as 64-pixel
-// TMA boxes {32 ch, TW, TH, 1} in the SWIZZLE_128B image; TF32 wgmma reads only K-major shared-memory operands, so this
-// kernel runs the warp-level TF32 MMA (mma.sync m16n8k8) with fragments gathered from the swizzled stage (conflict-free:
-// the swizzle spreads the 8 pixel rows a fragment touches over all banks). Split-K over pixel tiles across CTAs; partial sums
-// leave through fp32 reductions into the caller's gradient buffer (any strides). Extras in the epilogue, all on the
-// out-channel rows (swap = 0 only):
+// the roles (needs 128 | M-channels). GEMM with K = pixels on TF32 wgmma. Both operands arrive channel-contiguous (MN-major)
+// as 32-pixel TMA boxes {32 ch, TW, TH, 1} in the SWIZZLE_128B image ([32 px][128 B], 16-byte chunk c of pixel row p stored
+// at chunk c ^ (p & 7)), and TF32 wgmma reads only K-major shared-memory operands, so:
+//   * M (the CTA's 128 channels, 64 rows per MMA warpgroup) is the register operand (wgmma RS): the m64k8 A fragments are
+//     gathered from the stage with scalar loads;
+//   * N (NT <= 256 channels) is transposed by the MMA warps into a K-major SWIZZLE_128B image [NT rows][32 px], one 4 px x 4 ch
+//     micro-tile per thread and step (16-byte loads and stores). The image and the A fragments are double-buffered: the
+//     transpose of stage k + 1 runs while the wgmma of stage k is in flight.
+// Inside every 8-pixel group both operands use the K order  k-index kappa <-> pixel 2 (kappa % 4) + kappa / 4  (a sum over
+// pixels does not care about their order). An A-fragment load then reads pixels 2 tq (+1) of one parity, and the chunk swizzle
+// (p & 7) spreads the 32 lanes over all 32 banks; the micro-tile assignment below keeps the transpose conflict-free as well.
+// Split-K over pixel tiles across CTAs; partial sums leave through fp32 reductions into the caller's gradient buffer (any
+// strides). Extras in the epilogue, all on the M rows (colsum any mode, the BatchNorm terms swap = 0 only):
 //   * eval-BatchNorm scale: dW[co] = sc[co] * sum gm X  (gm = the un-scaled masked gradient the data gradient also consumes)
 //   * dgamma[co] += rstd[co] * <W[co], sum gm X>        (d/dgamma of BN(conv(x)) without touching any activation)
-//   * grouped convolutions: only the diagonal 128-channel blocks are computed and only in-group entries leave.
-constexpr int kWgStages = 2;                      // 2 x 96 KB: the stage ring fills the shared memory
-constexpr int kWgPx = 64;                         // pixels (K) per stage
-constexpr int kWgBox = kWgPx * 128;               // bytes of one {32 ch, 64 px} box
+//   * colsum[m] += sum over pixels of the M operand, summed from the A fragments (CTAs of the first tap and N tile)
+//   * grouped convolutions: only diagonal blocks are computed and only in-group entries leave. When the group size divides 64
+//     (G64), each warpgroup computes its own 64 x 64 diagonal block; otherwise both compute their half of the 128 x 128 block.
+constexpr int kWgStages = 3;
+constexpr int kWgPx = 32;                         // pixels (K) per stage
+constexpr int kWgBox = kWgPx * 128;               // bytes of one {32 ch, 32 px} box
 constexpr int kWgStageBytes = (4 + 8) * kWgBox;   // M: 128 channels, N: up to 256 channels
-constexpr int kWgOffBar = kWgStages * kWgStageBytes;
+constexpr int kWgImgBytes = 256 * 128;            // K-major N image: up to 256 rows of 32 pixels
+constexpr int kWgOffImg = kWgStages * kWgStageBytes;
+constexpr int kWgOffBar = kWgOffImg + 2 * kWgImgBytes;
 constexpr size_t kWgSmem = (size_t)kWgOffBar + 256;
-constexpr int kWgThreads = 288;                   // 8 MMA warps (2 along M x 4 along N) + 1 TMA producer warp
+constexpr int kWgThreads = 384;                   // TMA producer warpgroup, two MMA warpgroups
 
 struct WgradParams {
   float* dw;
@@ -437,10 +450,9 @@ struct WgradParams {
   int N, OH, OW;                   // pixel grid of gy
   int Mch, Nch;                    // channel counts of the two operands
   int ntaps, ksize, stride, swap;
-  int TW, TH, tiles_w, tiles_h;    // 64-pixel tiles
-  int NT;                          // N channels per output tile (multiple of 32)
+  int TW, TH, tiles_w, tiles_h;    // 32-pixel tiles
   int ksplit;
-  int cpg;                         // > 0: grouped (diagonal blocks, NT = 128)
+  int cpg;                         // > 0: grouped (diagonal blocks of 128 channels)
   const float* gamma;              // eval BatchNorm of the out-channels (or null)
   const float* var;
   float eps;
@@ -451,26 +463,19 @@ struct WgradParams {
   unsigned char wt[DVD_CONV_MAX_TAPS];
 };
 
-// element (px, ch) of a stage operand made of 32-channel boxes, each [64 px][128 B] SWIZZLE_128B
-__device__ __forceinline__ uint32_t wg_off(int px, int ch) {
-  return (uint32_t)(ch >> 5) * kWgBox + (uint32_t)px * 128u + ((((uint32_t)(ch & 31) >> 2) ^ ((uint32_t)px & 7u)) << 4) + (uint32_t)(ch & 3) * 4u;
-}
-__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
+template <int NT, bool G64>
 __global__ void __launch_bounds__(kWgThreads, 1) conv_wgrad_kernel(const __grid_constant__ CUtensorMap mapM,
                                                                   const __grid_constant__ CUtensorMap mapN,
                                                                   const __grid_constant__ WgradParams P) {
+  constexpr int WN = G64 ? 64 : NT;               // accumulator columns of one warpgroup
+  constexpr int kUnits = NT / 32 * 64;            // transpose micro-tiles of one stage's N operand
+  constexpr int kUnitSteps = (kUnits + 255) / 256;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kWgOffBar);
   uint64_t* full = bars;            // [kWgStages]
   uint64_t* empty = bars + 8;       // [kWgStages]: one arrival per MMA warp
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) __trap();   // swizzled stages need 1024-byte alignment
-  const int nb = P.NT / 32;                                   // 32-channel boxes of the N tile
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
+  if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) __trap();   // swizzled stages and images need 1024-byte alignment
   if (threadIdx.x == 0) {
     for (int i = 0; i < kWgStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 8); }
     fence_mbar_init();
@@ -481,21 +486,23 @@ __global__ void __launch_bounds__(kWgThreads, 1) conv_wgrad_kernel(const __grid_
   // this CTA: output tile (tap, 128 M-channels, NT N-channels) and a contiguous range of pixel tiles.
   // blockIdx.x = (tap, M block, N tile) * ksplit + part
   const int out_grp = blockIdx.x / P.ksplit, part = blockIdx.x - out_grp * P.ksplit;
-  const int n_m = P.Mch / 128, n_n = P.cpg ? 1 : P.Nch / P.NT;
+  const int n_m = P.Mch / 128, n_n = P.cpg ? 1 : P.Nch / NT;
   const int t = out_grp / (n_m * n_n);
   const int rem = out_grp - t * (n_m * n_n);
   const int m0 = (rem / n_n) * 128;
-  const int n0 = P.cpg ? m0 : (rem % n_n) * P.NT;
+  const int n0 = P.cpg ? m0 : (rem % n_n) * NT;
   const int dy = P.dy[t], dx = P.dx[t];
   // the CTAs of the first tap and first N tile also reduce their M operand over the pixels
   const bool do_colsum = P.colsum != nullptr && t == 0 && (P.cpg || rem % n_n == 0);
   const int px_tiles = P.N * P.tiles_h * P.tiles_w;
   const int per = (px_tiles + P.ksplit - 1) / P.ksplit;
   const int kt0 = part * per, kt1 = min(px_tiles, kt0 + per);
-  const uint32_t stage_tx = (uint32_t)(4 + nb) * kWgBox;
 
-  if (warp == 8) {
-    if (lane == 0) {
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    // ===== TMA producer =====
+    if (threadIdx.x == 0) {
+      const uint32_t stage_tx = (uint32_t)(4 + NT / 32) * kWgBox;
       uint32_t it = 0;
       for (int kt = kt0; kt < kt1; ++kt, ++it) {
         const uint32_t s = it % kWgStages, ph = (it / kWgStages) & 1u;
@@ -508,97 +515,147 @@ __global__ void __launch_bounds__(kWgThreads, 1) conv_wgrad_kernel(const __grid_
         mbar_wait(&empty[s], ph ^ 1u);
         mbar_arrive_expect_tx(&full[s], stage_tx);
         for (int j = 0; j < 4; ++j) tma_load_4d(st + j * kWgBox, &mapM, m0 + 32 * j, mw, mh, img, &full[s]);
-        for (int j = 0; j < nb; ++j) tma_load_4d(st + (4 + j) * kWgBox, &mapN, n0 + 32 * j, nw, nh, img, &full[s]);
+        for (int j = 0; j < NT / 32; ++j) tma_load_4d(st + (4 + j) * kWgBox, &mapN, n0 + 32 * j, nw, nh, img, &full[s]);
       }
     }
     return;
   }
+  setmaxnreg_inc<232>();
   if (kt1 <= kt0) return;
-  // warp (wm, wn): M rows [64 wm, 64 wm + 64) as four m16 tiles, N columns [wn * NT/4, ...) as nj8 = NT/32 n8 tiles
-  const int wm = warp >> 2, wn = warp & 3, g = lane >> 2, tq = lane & 3;
-  const int nj8 = P.NT / 32, nbase = wn * (P.NT / 4);
-  float c[4][8][4];
-  float cs[4][4];
+  // ===== MMA warpgroup cw: M rows [64 cw, 64 cw + 64) of the CTA's 128 =====
+  const int cw = wg - 1, et = threadIdx.x - 128;
+  const int g = lane >> 2, tq = lane & 3;
+  const int lrow = cw * 64 + (warp & 3) * 16 + g;     // this thread's fragment rows: lrow, lrow + 8
+  // A fragment of pixel group kk: a0 = (row lrow, pixel 8 kk + 2 tq), a1 = (lrow + 8, same pixel), a2 / a3 = pixel 8 kk + 2 tq + 1
+  uint32_t a_off[2][2];                               // [row + 8?][pixel parity], byte offsets in the stage's M part
 #pragma unroll
-  for (int mi = 0; mi < 4; ++mi) {
+  for (int h = 0; h < 2; ++h)
 #pragma unroll
-    for (int nj = 0; nj < 8; ++nj)
+    for (int e = 0; e < 2; ++e) {
+      const uint32_t ch = (uint32_t)(lrow + 8 * h), px = (uint32_t)(2 * tq + e);
+      a_off[h][e] = (ch >> 5) * kWgBox + px * 128u + ((((ch & 31u) >> 2) ^ px) << 4) + (ch & 3u) * 4u;
+    }
+  // transpose micro-tiles: unit u = (32-channel box j, l = 8 hi + tt) covers channels 32 j + 4 tt .. + 3 and K chunk
+  // q = (tt >> 1) ^ hi, i.e. pixels 8 (q >> 1) + 2 e + (q & 1), e = 0..3. Within every 8 lanes both the loads (pixel rows,
+  // chunk tt ^ (p & 7)) and the stores (channel rows, chunk q ^ (n & 7)) hit 8 different 16-byte bank groups.
+  uint32_t u_src[kUnitSteps], u_dst[kUnitSteps];
 #pragma unroll
-      for (int e = 0; e < 4; ++e) c[mi][nj][e] = 0.f;
-#pragma unroll
-    for (int e = 0; e < 4; ++e) cs[mi][e] = 0.f;
+  for (int r = 0; r < kUnitSteps; ++r) {
+    const uint32_t u = (uint32_t)(et + 256 * r), j = u >> 6, tt = u & 7u, hi = (u >> 3) & 7u, q = (tt >> 1) ^ hi;
+    u_src[r] = 4u * kWgBox + j * kWgBox + (8u * (q >> 1) + (q & 1u)) * 128u;
+    u_dst[r] = (32u * j + 4u * tt) * 128u;
   }
-  const bool warp_cs = do_colsum && wn == 0;
-  const uint32_t one = __float_as_uint(1.0f);
-  uint32_t it = 0;
-  for (int kt = kt0; kt < kt1; ++kt, ++it) {
+  const uint32_t u_tt = (uint32_t)et & 7u, u_q = (u_tt >> 1) ^ (((uint32_t)et >> 3) & 7u);
+  const uint32_t img0 = smem_u32(smem + kWgOffImg) + (G64 ? (uint32_t)cw * 64u * 128u : 0u);
+  float acc[WN / 2];
+#pragma unroll
+  for (int i = 0; i < WN / 2; ++i) acc[i] = 0.f;
+  uint32_t a[2][4][4];
+  float cs[2] = {0.f, 0.f};
+
+  // one stage into buffer B (fragments a[B], image B); on return its wgmma group is in flight
+  auto stage = [&](auto buf, uint32_t it) {
+    constexpr int B = decltype(buf)::value;
     const uint32_t s = it % kWgStages, ph = (it / kWgStages) & 1u;
     mbar_wait(&full[s], ph);
-    const uint8_t* sM = smem + (size_t)s * kWgStageBytes;
-    const uint8_t* sN = sM + 4 * kWgBox;
-#pragma unroll 2
-    for (int kk = 0; kk < kWgPx / 8; ++kk) {
-      const int p0 = kk * 8 + tq, p1 = p0 + 4;
-      uint32_t a[4][4];
+    const uint8_t* st = smem + (size_t)s * kWgStageBytes;
 #pragma unroll
-      for (int mi = 0; mi < 4; ++mi) {
-        const int m = wm * 64 + mi * 16 + g;
-        a[mi][0] = *reinterpret_cast<const uint32_t*>(sM + wg_off(p0, m));
-        a[mi][1] = *reinterpret_cast<const uint32_t*>(sM + wg_off(p0, m + 8));
-        a[mi][2] = *reinterpret_cast<const uint32_t*>(sM + wg_off(p1, m));
-        a[mi][3] = *reinterpret_cast<const uint32_t*>(sM + wg_off(p1, m + 8));
-      }
+    for (int kk = 0; kk < 4; ++kk) {
+      a[B][kk][0] = *reinterpret_cast<const uint32_t*>(st + a_off[0][0] + kk * 1024);
+      a[B][kk][1] = *reinterpret_cast<const uint32_t*>(st + a_off[1][0] + kk * 1024);
+      a[B][kk][2] = *reinterpret_cast<const uint32_t*>(st + a_off[0][1] + kk * 1024);
+      a[B][kk][3] = *reinterpret_cast<const uint32_t*>(st + a_off[1][1] + kk * 1024);
+    }
+    if (do_colsum) {
 #pragma unroll
-      for (int nj = 0; nj < 8; ++nj) {
-        if (nj < nj8) {
-          const int n = nbase + nj * 8 + g;
-          const uint32_t b0 = *reinterpret_cast<const uint32_t*>(sN + wg_off(p0, n));
-          const uint32_t b1 = *reinterpret_cast<const uint32_t*>(sN + wg_off(p1, n));
-#pragma unroll
-          for (int mi = 0; mi < 4; ++mi) mma_tf32(c[mi][nj], a[mi], b0, b1);
-        }
-      }
-      if (warp_cs) {
-#pragma unroll
-        for (int mi = 0; mi < 4; ++mi) mma_tf32(cs[mi], a[mi], one, one);
+      for (int kk = 0; kk < 4; ++kk) {
+        cs[0] += __uint_as_float(a[B][kk][0]) + __uint_as_float(a[B][kk][2]);
+        cs[1] += __uint_as_float(a[B][kk][1]) + __uint_as_float(a[B][kk][3]);
       }
     }
+    uint8_t* img = smem + kWgOffImg + B * kWgImgBytes;
+#pragma unroll
+    for (int r = 0; r < kUnitSteps; ++r) {
+      if (kUnits % 256 != 0 && et + 256 * r >= kUnits) continue;
+      float4 v[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const uint32_t p = 2u * e + (u_q & 1u);              // pixel row & 7
+        v[e] = *reinterpret_cast<const float4*>(st + u_src[r] + 256u * e + ((u_tt ^ p) << 4));
+      }
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const uint32_t n7 = (4u * u_tt + i) & 7u;            // channel row & 7
+        const float4 w = i == 0 ? make_float4(v[0].x, v[1].x, v[2].x, v[3].x)
+                       : i == 1 ? make_float4(v[0].y, v[1].y, v[2].y, v[3].y)
+                       : i == 2 ? make_float4(v[0].z, v[1].z, v[2].z, v[3].z)
+                                : make_float4(v[0].w, v[1].w, v[2].w, v[3].w);
+        *reinterpret_cast<float4*>(img + u_dst[r] + 128u * i + ((u_q ^ n7) << 4)) = w;
+      }
+    }
+    fence_proxy_async_smem();                                // the image is read by wgmma (async proxy)
     __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[s]);
+    if (lane == 0) mbar_arrive(&empty[s]);                   // stage fully consumed: fragments in registers, N in the image
+    wgmma_wait<0>();                                         // the previous stage's wgmma (other buffer) is done ...
+    named_sync(1, 256);                                      // ... in both warpgroups, and this image is complete
+    wgmma_fence();
+    const uint32_t ib = img0 + B * kWgImgBytes;
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_tf32_rs<WN>(acc, a[B][kk], make_sdesc_k_sw128(ib + kk * 32), 1u);
+    wgmma_commit();
+  };
+  const uint32_t n_it = (uint32_t)(kt1 - kt0);
+  uint32_t it = 0;
+  for (; it + 2 <= n_it; it += 2) {
+    stage(std::integral_constant<int, 0>{}, it);
+    stage(std::integral_constant<int, 1>{}, it + 1);
   }
-  // epilogue: fragment c[mi][nj] holds rows m0 + 64 wm + 16 mi + g (+8), columns n0 + nbase + 8 nj + 2 tq (+1)
+  if (it < n_it) stage(std::integral_constant<int, 0>{}, it);
+  wgmma_wait<0>();
+  fence_regs(acc);
+
+  // epilogue: acc[4 j + 2 h + e] holds row lrow + 8 h, column noff + 8 j + 2 tq + e of the CTA's (128 x NT) tile
+  const int noff = G64 ? cw * 64 : 0;
   const int wt = P.wt[t];
   const long tap_off = (long)(wt / P.ksize) * P.s_ky + (long)(wt % P.ksize) * P.s_kx;
-#pragma unroll
-  for (int mi = 0; mi < 4; ++mi) {
+  if (do_colsum) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int lm = wm * 64 + mi * 16 + g + 8 * h, m = m0 + lm;
-      float* dst = P.dw + (long)m * P.s_m + tap_off;
-      const float* wrow = P.w ? P.w + (long)m * P.s_m + tap_off : nullptr;
-      float sc = 1.f, rstd = 0.f;
-      if (P.gamma) {
-        rstd = rsqrtf(__ldg(P.var + m) + P.eps);
-        sc = __ldg(P.gamma + m) * rstd;
-      }
-      float dot = 0.f;
+      cs[h] += __shfl_xor_sync(0xffffffffu, cs[h], 1);
+      cs[h] += __shfl_xor_sync(0xffffffffu, cs[h], 2);
+    }
+  }
 #pragma unroll
-      for (int nj = 0; nj < 8; ++nj) {
-        if (nj >= nj8) continue;
+  for (int h = 0; h < 2; ++h) {
+    const int lm = lrow + 8 * h, m = m0 + lm;
+    float* dst = P.dw + (long)m * P.s_m + tap_off;
+    const float* wrow = P.w ? P.w + (long)m * P.s_m + tap_off : nullptr;
+    float sc = 1.f, rstd = 0.f;
+    if (P.gamma) {
+      rstd = rsqrtf(__ldg(P.var + m) + P.eps);
+      sc = __ldg(P.gamma + m) * rstd;
+    }
+    float dot = 0.f;
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int ln = nbase + nj * 8 + 2 * tq + e;
-          if (P.cpg && ln / P.cpg != lm / P.cpg) continue;        // grouped: in-group entries of the diagonal block only
-          const long o = (long)(P.cpg ? ln % P.cpg : n0 + ln) * P.s_n;
-          const float v = c[mi][nj][2 * h + e];
-          if (wrow) dot = fmaf(v, __ldg(wrow + o), dot);
-          atomicAdd(dst + o, v * sc);
-        }
+    for (int j = 0; j < WN / 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int ln = noff + j * 8 + 2 * tq + e;
+        if (P.cpg && ln / P.cpg != lm / P.cpg) continue;        // grouped: in-group entries of the diagonal block only
+        const long o = (long)(P.cpg ? ln % P.cpg : n0 + ln) * P.s_n;
+        const float v = acc[4 * j + 2 * h + e];
+        if (wrow) dot = fmaf(v, __ldg(wrow + o), dot);
+        atomicAdd(dst + o, v * sc);
       }
-      if (warp_cs && tq == 0) {
-        const float csum = cs[mi][2 * h];            // every column of the ones-product holds the column sum
-        atomicAdd(P.colsum + m, csum);
-        if (P.dgamma && P.mean) dot = fmaf(-__ldg(P.mean + m), csum, dot);      // d gamma = rstd * (<W, dW> - mean * sum gm)
+    }
+    if (P.dgamma) {
+      dot += __shfl_xor_sync(0xffffffffu, dot, 1);
+      dot += __shfl_xor_sync(0xffffffffu, dot, 2);
+    }
+    if (tq == 0) {
+      if (do_colsum) {
+        atomicAdd(P.colsum + m, cs[h]);
+        if (P.dgamma && P.mean) dot = fmaf(-__ldg(P.mean + m), cs[h], dot);   // d gamma = rstd * (<W, dW> - mean * sum gm)
       }
       if (P.dgamma) atomicAdd(P.dgamma + m, dot * rstd);
     }
@@ -690,6 +747,21 @@ int launch_conv(const CUtensorMap& mapA, const CUtensorMap& mapW, const ConvPara
   if (int e = per_device_attr((const void*)conv2d_tc_kernel<NT>, kSmem, attr_done)) return e;
   DVD_CUDA_CALL(dvd::launch(conv2d_tc_kernel<NT>, grid, kThreads, kSmem, st, mapA, mapW, P));
   DVD_CUDA_LAUNCH_CHECK("conv2d_tc_kernel");
+  return 0;
+}
+
+template <int NT, bool G64>
+int launch_wgrad(const CUtensorMap& mapM, const CUtensorMap& mapN, WgradParams P, int out_tiles, int px_tiles, cudaStream_t st) {
+  static bool attr_done[16] = {};
+  if (int e = per_device_attr((const void*)conv_wgrad_kernel<NT, G64>, kWgSmem, attr_done)) return e;
+  // split-K so that all CTAs are resident in ONE wave (a second, nearly empty wave would double the time)
+  const int resident = max_clusters(conv_wgrad_kernel<NT, G64>, kWgThreads, kWgSmem, 1);
+  int ksplit = resident / out_tiles;
+  if (ksplit > px_tiles) ksplit = px_tiles;
+  if (ksplit < 1) ksplit = 1;
+  P.ksplit = ksplit;
+  DVD_CUDA_CALL(dvd::launch(conv_wgrad_kernel<NT, G64>, out_tiles * ksplit, kWgThreads, kWgSmem, st, mapM, mapN, P));
+  DVD_CUDA_LAUNCH_CHECK("conv_wgrad_kernel");
   return 0;
 }
 
@@ -902,19 +974,20 @@ extern "C" int dvd_conv2d_wgrad(const dvd_conv_desc* desc, const float* x, const
   P.gamma = bn_gamma; P.var = bn_var; P.eps = d.bn_eps; P.dgamma = dgamma; P.colsum = colsum; P.mean = bn_mean;
   for (int t = 0; t < d.ntaps; ++t) { P.dy[t] = d.dy[t]; P.dx[t] = d.dx[t]; P.wt[t] = d.wt[t]; }
   const int Cin = d.Cin, Cout = d.Cout;
+  int NT;                          // N channels per output tile (multiple of 32)
   if (groups > 1) {
     P.cpg = Cin / groups;
     if (Cin != Cout || Cin % 128 != 0 || 128 % P.cpg != 0) {
       set_error("dvd_conv2d_wgrad: grouped needs Cin == Cout, 128 | C and cpg | 128 (C=%d groups=%d)", Cin, groups);
       return -2;
     }
-    P.swap = 0; P.Mch = Cout; P.Nch = Cin; P.NT = 128;
+    P.swap = 0; P.Mch = Cout; P.Nch = Cin; NT = 128;
     P.s_m = stride_co; P.s_n = stride_ci;
   } else if (Cout % 128 == 0 && Cin % 32 == 0 && (Cin <= 256 || Cin % 256 == 0)) {
-    P.swap = 0; P.Mch = Cout; P.Nch = Cin; P.NT = Cin >= 256 ? 256 : Cin;
+    P.swap = 0; P.Mch = Cout; P.Nch = Cin; NT = Cin >= 256 ? 256 : Cin;
     P.s_m = stride_co; P.s_n = stride_ci;
   } else if (Cin % 128 == 0 && Cout % 32 == 0 && (Cout <= 256 || Cout % 256 == 0) && !bn_gamma) {
-    P.swap = 1; P.Mch = Cin; P.Nch = Cout; P.NT = Cout >= 256 ? 256 : Cout;
+    P.swap = 1; P.Mch = Cin; P.Nch = Cout; NT = Cout >= 256 ? 256 : Cout;
     P.s_m = stride_ci; P.s_n = stride_co;
     DVD_ARG_CHECK(colsum == nullptr, "column sums are not available with swapped operands (Cout %% 128 != 0): use dvd_relu_bwd_colsum");
   } else {
@@ -935,23 +1008,25 @@ extern "C" int dvd_conv2d_wgrad(const dvd_conv_desc* desc, const float* x, const
   }
   P.tiles_w = (OW + P.TW - 1) / P.TW;
   P.tiles_h = (OH + P.TH - 1) / P.TH;
-  const int out_tiles = d.ntaps * (P.Mch / 128) * (P.cpg ? 1 : P.Nch / P.NT);
+  const int out_tiles = d.ntaps * (P.Mch / 128) * (P.cpg ? 1 : P.Nch / NT);
   const int px_tiles = N * P.tiles_h * P.tiles_w;
-  static bool attr_done[16] = {};
-  if (int e = per_device_attr((const void*)conv_wgrad_kernel, kWgSmem, attr_done)) return e;
-  // split-K so that all CTAs are resident in ONE wave (a second, nearly empty wave would double the time)
-  const int resident = max_clusters(conv_wgrad_kernel, kWgThreads, kWgSmem, 1);
-  int ksplit = resident / out_tiles;
-  if (ksplit > px_tiles) ksplit = px_tiles;
-  if (ksplit < 1) ksplit = 1;
-  P.ksplit = ksplit;
   CUtensorMap mapG, mapX;
   if (int e = make_nhwc_map(&mapG, gy, N, OH, OW, Cout, P.TW, P.TH, 1, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
   if (int e = make_nhwc_map(&mapX, x, N, H, W, Cin, P.TW, P.TH, d.stride, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
-  dvd::launch(conv_wgrad_kernel, out_tiles * ksplit, kWgThreads, kWgSmem, (cudaStream_t)stream, P.swap ? mapX : mapG,
-              P.swap ? mapG : mapX, P);
-  DVD_CUDA_LAUNCH_CHECK("conv_wgrad_kernel");
-  return 0;
+  const CUtensorMap& mapM = P.swap ? mapX : mapG;
+  const CUtensorMap& mapN = P.swap ? mapG : mapX;
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (P.cpg && 64 % P.cpg == 0) return launch_wgrad<128, true>(mapM, mapN, P, out_tiles, px_tiles, st);
+  switch (NT) {
+    case 32: return launch_wgrad<32, false>(mapM, mapN, P, out_tiles, px_tiles, st);
+    case 64: return launch_wgrad<64, false>(mapM, mapN, P, out_tiles, px_tiles, st);
+    case 96: return launch_wgrad<96, false>(mapM, mapN, P, out_tiles, px_tiles, st);
+    case 128: return launch_wgrad<128, false>(mapM, mapN, P, out_tiles, px_tiles, st);
+    case 160: return launch_wgrad<160, false>(mapM, mapN, P, out_tiles, px_tiles, st);
+    case 192: return launch_wgrad<192, false>(mapM, mapN, P, out_tiles, px_tiles, st);
+    case 224: return launch_wgrad<224, false>(mapM, mapN, P, out_tiles, px_tiles, st);
+    default: return launch_wgrad<256, false>(mapM, mapN, P, out_tiles, px_tiles, st);
+  }
 }
 
 /* resident CTAs of the two tensor-core kernels for cluster sizes 1, 2, 4 (diagnostic): out[0..2] forward / data gradient kernel,
@@ -959,11 +1034,11 @@ extern "C" int dvd_conv2d_wgrad(const dvd_conv_desc* desc, const float* x, const
 extern "C" int dvd_conv2d_cluster_info(int* out) {
   static bool a1[16] = {}, a2[16] = {};
   if (int e = per_device_attr((const void*)conv2d_tc_kernel<kMaxNT>, kSmem, a1)) return e;
-  if (int e = per_device_attr((const void*)conv_wgrad_kernel, kWgSmem, a2)) return e;
+  if (int e = per_device_attr((const void*)conv_wgrad_kernel<256, false>, kWgSmem, a2)) return e;
   const int cs[3] = {1, 2, 4};
   for (int i = 0; i < 3; ++i) {
     out[i] = cs[i] * max_clusters(conv2d_tc_kernel<kMaxNT>, kThreads, kSmem, cs[i]);
-    out[3 + i] = cs[i] * max_clusters(conv_wgrad_kernel, kWgThreads, kWgSmem, cs[i]);
+    out[3 + i] = cs[i] * max_clusters(conv_wgrad_kernel<256, false>, kWgThreads, kWgSmem, cs[i]);
   }
   return 0;
 }
