@@ -40,10 +40,16 @@ class PackItem(ctypes.Structure):
                 ('ksize', ctypes.c_int), ('groups', ctypes.c_int), ('kblock', ctypes.c_int), ('bn_eps', ctypes.c_float)]
 
 
+DVD_MLP_MAX_NIN = 256
+DVD_MLP_MAX_FREQ_XYZ = 42
+DVD_MLP_MAX_FREQ_T = 126
+
+
 class MlpCfg(ctypes.Structure):
     """struct dvd_mlp_cfg (include/dvd_b200.h)."""
     _fields_ = [('n_freq_xyz', ctypes.c_int), ('n_freq_t', ctypes.c_int), ('time_dependent', ctypes.c_int),
-                ('sf_mag_div', ctypes.c_float), ('freq_xyz', ctypes.c_float * 16), ('freq_t', ctypes.c_float * 16)]
+                ('sf_mag_div', ctypes.c_float), ('freq_xyz', ctypes.c_float * DVD_MLP_MAX_FREQ_XYZ),
+                ('freq_t', ctypes.c_float * DVD_MLP_MAX_FREQ_T)]
 
 
 _I, _F, _P = ctypes.c_int, ctypes.c_float, ctypes.c_void_p

@@ -37,7 +37,7 @@ int num_sms() {
 }  // namespace dvd
 
 extern "C" const char* dvd_last_error(void) { return dvd::g_err; }
-extern "C" int dvd_version(void) { return 100; }
+extern "C" int dvd_version(void) { return 101; }
 /* sizes of the structs that cross the C ABI by pointer (which: 0 dvd_loss_cfg, 1 dvd_mlp_cfg, 2 dvd_conv_desc, 3 dvd_pack_item):
  * a binding in another language checks its own layout against these */
 extern "C" long dvd_struct_size(int which) {

@@ -35,6 +35,12 @@ __host__ __device__ inline int mlp_nin(const dvd_mlp_cfg& c) {
   int nt = c.time_dependent ? (1 + 2 * c.n_freq_t) : 0;
   return nt + 3 + 6 * c.n_freq_xyz;
 }
+// (16, 16, time-dependent) and (16, time-independent): the two configurations whose kernels are compiled for their counts.
+// Their first layer is padded to a multiple of 16 input channels; every other configuration runs the generic kernels and
+// pads it to a multiple of 64, so that its data-gradient MMA width (N = kpad0) takes one of four values.
+__host__ __device__ inline bool mlp_specialised(const dvd_mlp_cfg& c) {
+  return c.n_freq_xyz == 16 && (!c.time_dependent || c.n_freq_t == 16);
+}
 __host__ __device__ inline int rows_f(int l) { return l < 5 ? kWidth : 16; }
 __host__ __device__ inline int rows_b(const MlpLayout& L, int l) { return l == 0 ? L.kpad0 : kWidth; }
 __host__ __device__ inline int nkc_f(const MlpLayout& L, int l) { return l == 0 ? L.k0_chunks : 4; }
@@ -62,7 +68,7 @@ __host__ __device__ inline int layer_out(int l) { return l == 5 ? 3 : kWidth; }
 inline MlpLayout make_layout(const dvd_mlp_cfg& c, long npx) {
   MlpLayout L;
   L.nin = mlp_nin(c);
-  L.kpad0 = (L.nin + 15) / 16 * 16;
+  L.kpad0 = mlp_specialised(c) ? (L.nin + 15) / 16 * 16 : (L.nin + 63) / 64 * 64;
   L.k0_chunks = (L.kpad0 + 63) / 64;
   L.npx = npx;
   L.ntiles = (npx + kTileM - 1) / kTileM;

@@ -78,31 +78,36 @@ __global__ void __launch_bounds__(256) pack_weights_kernel(PackParams P) {
 //   xyz_emb = [x, y, z, cos(f_k x), cos(f_k y), cos(f_k z) k<FX, sin(...) k<FX]
 // Loops over the frequencies are deliberately NOT unrolled: a fully unrolled epilogue was ~0.5 MB of SASS and
 // spent 30 % of its issue slots waiting for the instruction cache.
+// FX = kRuntime: the generic kernels; the counts and time_dependent are read from the configuration (FT, TD unused).
+constexpr int kRuntime = -1;
 template <int FX, int FT, bool TD>
 struct Embed {
-  static constexpr int NT = TD ? 1 + 2 * FT : 0;
-  static constexpr int NIN = NT + 3 + 6 * FX;
-  static constexpr int KPAD = (NIN + 15) / 16 * 16;
-  // fast path: cos block starts at an even feature index, so two frequencies give exactly three packed words
-  static constexpr bool kPaired = ((NT + 3) % 2 == 0) && (FX % 2 == 0);
+  static constexpr bool kStatic = FX != kRuntime;
+  static constexpr int KPAD = kStatic ? ((TD ? 1 + 2 * FT : 0) + 3 + 6 * FX + 15) / 16 * 16 : 0;
+  int fx, ft, nt;
+  bool td;
+  __device__ __forceinline__ explicit Embed(const dvd_mlp_cfg& c)
+      : fx(kStatic ? FX : c.n_freq_xyz), ft(kStatic ? FT : c.n_freq_t), td(kStatic ? TD : c.time_dependent != 0) {
+    nt = td ? 1 + 2 * ft : 0;
+  }
 
   // feature j (runtime index)
-  static __device__ __forceinline__ float feature(const dvd_mlp_cfg& c, int j, float t, float x, float y, float z) {
+  __device__ __forceinline__ float feature(const dvd_mlp_cfg& c, int j, float t, float x, float y, float z) const {
     float s, co;
-    if (j < NT) {
+    if (j < nt) {
       if (j == 0) return t;
       int k = j - 1;
-      const bool is_sin = k >= FT;
-      if (is_sin) k -= FT;
+      const bool is_sin = k >= ft;
+      if (is_sin) k -= ft;
       fast_sincos(c.freq_t[k] * t, s, co);
       return is_sin ? s : co;
     }
-    j -= NT;
+    j -= nt;
     if (j < 3) return j == 0 ? x : (j == 1 ? y : z);
     j -= 3;
-    if (j >= 6 * FX) return 0.f;
-    const bool is_sin = j >= 3 * FX;
-    if (is_sin) j -= 3 * FX;
+    if (j >= 6 * fx) return 0.f;
+    const bool is_sin = j >= 3 * fx;
+    if (is_sin) j -= 3 * fx;
     const int k = j / 3, d = j - 3 * k;
     fast_sincos(c.freq_xyz[k] * (d == 0 ? x : (d == 1 ? y : z)), s, co);
     return is_sin ? s : co;
@@ -237,10 +242,12 @@ struct FwdParams {
 template <int FX, int FT, bool TD, bool SAVE>
 __global__ void __launch_bounds__(kThreadsMlp, 1) mlp_chain_fwd_kernel(const __grid_constant__ FwdParams P) {
   using E = Embed<FX, FT, TD>;
+  const E emb(P.cfg);
   extern __shared__ uint8_t smem_raw[];
   ChainSmem S = carve(smem_raw);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
   const MlpLayout& L = P.L;
+  const int kpad0 = E::kStatic ? E::KPAD : L.kpad0;
   chain_setup(S);
   DVD_PDL_ENTER();               // barriers are set up: now wait for the producer of the operands
   for (int i = threadIdx.x; i < 5 * 256 + 16; i += blockDim.x) S.bias[i] = P.bias[i];
@@ -271,7 +278,7 @@ __global__ void __launch_bounds__(kThreadsMlp, 1) mlp_chain_fwd_kernel(const __g
       px[h] = py[h] = pz[h] = tt[h] = 0.f;
       if (valid[h]) {
         px[h] = P.p0[pidx[h]]; py[h] = P.p0[pidx[h] + P.hw]; pz[h] = P.p0[pidx[h] + 2 * P.hw];
-        if (TD) tt[h] = P.t0[(size_t)b * P.hw + i];
+        if (emb.td) tt[h] = P.t0[(size_t)b * P.hw + i];
       }
     }
     for (int e = 0; e < P.n_eval; ++e) {
@@ -284,11 +291,11 @@ __global__ void __launch_bounds__(kThreadsMlp, 1) mlp_chain_fwd_kernel(const __g
           float* ps = P.p_steps + (size_t)e * P.npx * 3 + pidx[h];
           ps[0] = px[h]; ps[P.hw] = py[h]; ps[2 * P.hw] = pz[h];
         }
-        uint8_t* x0_hi = SAVE ? save_e + L.xs_off[0] + (size_t)chunk * blk_bytes(E::KPAD) : nullptr;
+        uint8_t* x0_hi = SAVE ? save_e + L.xs_off[0] + (size_t)chunk * blk_bytes(kpad0) : nullptr;
 #pragma unroll 1
         for (int w = t4; w < 32 * L.k0_chunks; w += 4) {        // features, then zeros up to the end of the last 64-K block
           uint32_t hi, lo;
-          split2(E::feature(P.cfg, 2 * w, tt[h], px[h], py[h], pz[h]), E::feature(P.cfg, 2 * w + 1, tt[h], px[h], py[h], pz[h]), hi, lo);
+          split2(emb.feature(P.cfg, 2 * w, tt[h], px[h], py[h], pz[h]), emb.feature(P.cfg, 2 * w + 1, tt[h], px[h], py[h], pz[h]), hi, lo);
           put_act(act, row, 2 * w, hi, lo);
           if (SAVE) *reinterpret_cast<uint32_t*>(x0_hi + act_offset(2 * w, row)) = hi;
         }
@@ -380,9 +387,12 @@ struct DgradParams {
   dvd_mlp_cfg cfg;
 };
 
-template <int FX, int FT, bool TD>
+// KPAD: the layer-0 width L.kpad0 (the N of its MMA)
+template <int FX, int FT, bool TD, int KPAD>
 __global__ void __launch_bounds__(kThreadsMlp, 1) mlp_dgrad_kernel(const __grid_constant__ DgradParams P) {
   using E = Embed<FX, FT, TD>;
+  static_assert(!E::kStatic || KPAD == E::KPAD, "layer-0 width of a specialised configuration");
+  const E emb(P.cfg);
   extern __shared__ uint8_t smem_raw[];
   ChainSmem S = carve(smem_raw);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
@@ -471,47 +481,99 @@ __global__ void __launch_bounds__(kThreadsMlp, 1) mlp_dgrad_kernel(const __grid_
     }
     // MMA(0) -> gradient w.r.t. the embedding; contract with d(embed)/d(xyz)
     {
-      float a0[E::KPAD / 2];
-      chain_layer<E::KPAD>(S, a0, act_u, nkc_b(0), it);
-      constexpr int CB = E::NT + 3, SB = E::NT + 3 + 3 * FX;   // first cos / sin feature
+      float a0[KPAD / 2];
+      chain_layer<KPAD>(S, a0, act_u, nkc_b(0), it);
+      if constexpr (E::kStatic) {
+        const int CB = emb.nt + 3, SB = emb.nt + 3 + 3 * emb.fx;   // first cos / sin feature
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        size_t pidx = 0;
-        const bool valid = pixel(h, pidx);
-        float p[3] = {0.f, 0.f, 0.f};
-        if (valid) {
-          p[0] = P.p_e[pidx]; p[1] = P.p_e[pidx + P.hw]; p[2] = P.p_e[pidx + 2 * P.hw];
-        }
-        float gp[3] = {0.f, 0.f, 0.f};
+        for (int h = 0; h < 2; ++h) {
+          size_t pidx = 0;
+          const bool valid = pixel(h, pidx);
+          float p[3] = {0.f, 0.f, 0.f};
+          if (valid) {
+            p[0] = P.p_e[pidx]; p[1] = P.p_e[pidx + P.hw]; p[2] = P.p_e[pidx + 2 * P.hw];
+          }
+          float gp[3] = {0.f, 0.f, 0.f};
 #pragma unroll
-        for (int j = 0; j < E::KPAD / 8; ++j) {
+          for (int j = 0; j < KPAD / 8; ++j) {
 #pragma unroll
-          for (int cc = 0; cc < 2; ++cc) {
-            const int c = 8 * j + 2 * t4 + cc;
-            const float gv = a0[4 * j + 2 * h + cc];
-            if (c >= E::NT && c < CB) {
-              gp[c - E::NT] += gv;
-            } else if (c >= CB && c < SB + 3 * FX) {
-              const bool is_sin = c >= SB;
-              const int k = (c - (is_sin ? SB : CB)) / 3, d = (c - (is_sin ? SB : CB)) % 3;
-              const float f = P.cfg.freq_xyz[k];
-              float s, co;
-              fast_sincos(f * p[d], s, co);
-              // d/dx cos(f x) = -f sin(f x) ; d/dx sin(f x) = f cos(f x)
-              gp[d] += is_sin ? f * co * gv : -f * s * gv;
+            for (int cc = 0; cc < 2; ++cc) {
+              const int c = 8 * j + 2 * t4 + cc;
+              const float gv = a0[4 * j + 2 * h + cc];
+              if (c >= emb.nt && c < CB) {
+                gp[c - emb.nt] += gv;
+              } else if (c >= CB && c < SB + 3 * emb.fx) {
+                const bool is_sin = c >= SB;
+                const int k = (c - (is_sin ? SB : CB)) / 3, d = (c - (is_sin ? SB : CB)) % 3;
+                const float f = P.cfg.freq_xyz[k];
+                float s, co;
+                fast_sincos(f * p[d], s, co);
+                // d/dx cos(f x) = -f sin(f x) ; d/dx sin(f x) = f cos(f x)
+                gp[d] += is_sin ? f * co * gv : -f * s * gv;
+              }
+            }
+          }
+#pragma unroll
+          for (int d = 0; d < 3; ++d) {
+            gp[d] += __shfl_xor_sync(0xffffffffu, gp[d], 1);
+            gp[d] += __shfl_xor_sync(0xffffffffu, gp[d], 2);
+          }
+          if (valid && P.a_out && t4 == 0) {
+#pragma unroll
+            for (int d = 0; d < 3; ++d) {
+              const size_t o = pidx + (size_t)d * P.hw;
+              P.a_out[o] = (P.a_in ? P.a_in[o] : 0.f) + gp[d];
             }
           }
         }
+      } else {
+        // Runtime counts: a0 goes to this warpgroup's activation image (free once every warp's layer-0 MMAs are done), one
+        // fp32 slot per thread and accumulator register (KPAD / 2 x 128 x 4 B <= kActBytes, conflict-free). Each thread then
+        // walks its own features in a loop that is not unrolled, so no array is indexed by a run-time value.
+        named_sync(1 + cw, 128);
+        float* g0 = reinterpret_cast<float*>(act) + (threadIdx.x & 127);
 #pragma unroll
-        for (int d = 0; d < 3; ++d) {
-          gp[d] += __shfl_xor_sync(0xffffffffu, gp[d], 1);
-          gp[d] += __shfl_xor_sync(0xffffffffu, gp[d], 2);
-        }
-        if (valid && P.a_out && t4 == 0) {
+        for (int i = 0; i < KPAD / 2; ++i) g0[i * 128] = a0[i];
+        const int nxyz = 3 + 6 * emb.fx, nj = (emb.nt + nxyz + 7) / 8;
+        for (int h = 0; h < 2; ++h) {
+          size_t pidx = 0;
+          const bool valid = pixel(h, pidx);
+          const float x = valid ? P.p_e[pidx] : 0.f, y = valid ? P.p_e[pidx + P.hw] : 0.f, z = valid ? P.p_e[pidx + 2 * P.hw] : 0.f;
+          float gx = 0.f, gy = 0.f, gz = 0.f;
+#pragma unroll 1
+          for (int j = 0; j < nj; ++j) {
 #pragma unroll
-          for (int d = 0; d < 3; ++d) {
-            const size_t o = pidx + (size_t)d * P.hw;
-            P.a_out[o] = (P.a_in ? P.a_in[o] : 0.f) + gp[d];
+            for (int cc = 0; cc < 2; ++cc) {
+              int q = 8 * j + 2 * t4 + cc - emb.nt;          // index into xyz_emb
+              if (q < 0 || q >= nxyz) continue;
+              const float gv = g0[(4 * j + 2 * h + cc) * 128];
+              float term = gv;
+              int d = q;
+              if (q >= 3) {
+                q -= 3;
+                const bool is_sin = q >= 3 * emb.fx;
+                if (is_sin) q -= 3 * emb.fx;
+                const int k = q / 3;
+                d = q - 3 * k;
+                const float f = P.cfg.freq_xyz[k];
+                float sn, co;
+                fast_sincos(f * (d == 0 ? x : (d == 1 ? y : z)), sn, co);
+                // d/dx cos(f x) = -f sin(f x) ; d/dx sin(f x) = f cos(f x)
+                term = is_sin ? f * co * gv : -f * sn * gv;
+              }
+              gx += d == 0 ? term : 0.f;
+              gy += d == 1 ? term : 0.f;
+              gz += d == 2 ? term : 0.f;
+            }
+          }
+          gx += __shfl_xor_sync(0xffffffffu, gx, 1); gx += __shfl_xor_sync(0xffffffffu, gx, 2);
+          gy += __shfl_xor_sync(0xffffffffu, gy, 1); gy += __shfl_xor_sync(0xffffffffu, gy, 2);
+          gz += __shfl_xor_sync(0xffffffffu, gz, 1); gz += __shfl_xor_sync(0xffffffffu, gz, 2);
+          if (valid && P.a_out && t4 == 0) {
+            const size_t o = pidx, o1 = pidx + P.hw, o2 = pidx + 2 * P.hw;
+            P.a_out[o] = (P.a_in ? P.a_in[o] : 0.f) + gx;
+            P.a_out[o1] = (P.a_in ? P.a_in[o1] : 0.f) + gy;
+            P.a_out[o2] = (P.a_in ? P.a_in[o2] : 0.f) + gz;
           }
         }
       }
@@ -642,8 +704,11 @@ __global__ void __launch_bounds__(kThreadsWgrad, 1) mlp_wgrad_kernel(const __gri
   const uint32_t so = smem_u32(ones);
   switch (J.n) {
     case 256: wgrad_consume<256>(J, stage, full, empty, so, q0, q1); break;
+    case 192: wgrad_consume<192>(J, stage, full, empty, so, q0, q1); break;
     case 144: wgrad_consume<144>(J, stage, full, empty, so, q0, q1); break;
+    case 128: wgrad_consume<128>(J, stage, full, empty, so, q0, q1); break;
     case 112: wgrad_consume<112>(J, stage, full, empty, so, q0, q1); break;
+    case 64: wgrad_consume<64>(J, stage, full, empty, so, q0, q1); break;
     case 16: wgrad_consume<16>(J, stage, full, empty, so, q0, q1); break;
     default: __trap();   // dvd_mlp_wgrad only builds jobs of these widths (checked there as well)
   }
@@ -691,13 +756,17 @@ __global__ void __launch_bounds__(256) acc_reg_final_kernel(const float* __restr
 }
 
 // =============================================================================================
+// variant 0: (16, 16, time-dependent), 1: (16, time-independent), 2: the generic kernels
 static int check_cfg_supported(const dvd_mlp_cfg* cfg, int* variant) {
   DVD_ARG_CHECK(cfg != nullptr, "null mlp cfg");
   if (cfg->time_dependent && cfg->n_freq_xyz == 16 && cfg->n_freq_t == 16) { *variant = 0; return 0; }
   if (!cfg->time_dependent && cfg->n_freq_xyz == 16) { *variant = 1; return 0; }
-  set_error("unsupported scene-flow MLP configuration (n_freq_xyz=%d n_freq_t=%d time_dependent=%d): the "
-            "tensor-core kernels are instantiated for n_freq_xyz=16 with (time_dependent, n_freq_t=16) or "
-            "(not time_dependent)", cfg->n_freq_xyz, cfg->n_freq_t, cfg->time_dependent);
+  const bool counts_ok = cfg->n_freq_xyz >= 0 && (!cfg->time_dependent || cfg->n_freq_t >= 0);
+  if (counts_ok && mlp_nin(*cfg) <= DVD_MLP_MAX_NIN) { *variant = 2; return 0; }
+  set_error("unsupported scene-flow MLP configuration (n_freq_xyz=%d n_freq_t=%d time_dependent=%d): the first layer "
+            "reads (time_dependent ? 1 + 2 n_freq_t : 0) + 3 + 6 n_freq_xyz = %d input features; the kernels take "
+            "non-negative counts and at most %d features", cfg->n_freq_xyz, cfg->n_freq_t, cfg->time_dependent,
+            mlp_nin(*cfg), DVD_MLP_MAX_NIN);
   return -2;
 }
 
@@ -775,7 +844,17 @@ extern "C" int dvd_mlp_chain_fwd(const dvd_mlp_cfg* cfg, const void* packed_fwd,
   P.save = (uint8_t*)save; P.npx = npx; P.hw = hw; P.L = make_layout(*cfg, npx); P.cfg = *cfg;
   cudaStream_t st = (cudaStream_t)stream;
   if (variant == 0) return launch_fwd<16, 16, true>(P, save != nullptr, st);
-  return launch_fwd<16, 0, false>(P, save != nullptr, st);
+  if (variant == 1) return launch_fwd<16, 0, false>(P, save != nullptr, st);
+  return launch_fwd<kRuntime, 0, false>(P, save != nullptr, st);
+}
+
+template <int FX, int FT, bool TD, int KPAD>
+static int launch_dgrad(const DgradParams& P, cudaStream_t st) {
+  DVD_CUDA_CALL(cudaFuncSetAttribute(mlp_dgrad_kernel<FX, FT, TD, KPAD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)kChainSmemBytes));
+  dvd::launch(mlp_dgrad_kernel<FX, FT, TD, KPAD>, chain_grid(P.L.ntiles), kThreadsMlp, kChainSmemBytes, st, P);
+  DVD_CUDA_LAUNCH_CHECK("mlp_dgrad");
+  return 0;
 }
 
 extern "C" int dvd_mlp_dgrad(const dvd_mlp_cfg* cfg, const void* packed_bwd, const float* p_e, const float* t0, float dt,
@@ -793,18 +872,14 @@ extern "C" int dvd_mlp_dgrad(const dvd_mlp_cfg* cfg, const void* packed_bwd, con
   P.g_acc = g_acc; P.g_step = g_step; P.a_in = a_in; P.a_out = a_out; P.save_e = (const uint8_t*)save_e;
   P.dy = (uint8_t*)dy_scratch; P.g_bias5 = g_bias5; P.npx = npx; P.hw = hw; P.L = make_layout(*cfg, npx); P.cfg = *cfg;
   cudaStream_t st = (cudaStream_t)stream;
-  int grid = chain_grid(P.L.ntiles);
-  if (variant == 0) {
-    DVD_CUDA_CALL(cudaFuncSetAttribute(mlp_dgrad_kernel<16, 16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)kChainSmemBytes));
-    dvd::launch(mlp_dgrad_kernel<16, 16, true>, grid, kThreadsMlp, kChainSmemBytes, st, P);
-  } else {
-    DVD_CUDA_CALL(cudaFuncSetAttribute(mlp_dgrad_kernel<16, 0, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)kChainSmemBytes));
-    dvd::launch(mlp_dgrad_kernel<16, 0, false>, grid, kThreadsMlp, kChainSmemBytes, st, P);
+  if (variant == 0) return launch_dgrad<16, 16, true, Embed<16, 16, true>::KPAD>(P, st);
+  if (variant == 1) return launch_dgrad<16, 0, false, Embed<16, 0, false>::KPAD>(P, st);
+  switch (P.L.kpad0) {
+    case 64: return launch_dgrad<kRuntime, 0, false, 64>(P, st);
+    case 128: return launch_dgrad<kRuntime, 0, false, 128>(P, st);
+    case 192: return launch_dgrad<kRuntime, 0, false, 192>(P, st);
+    default: return launch_dgrad<kRuntime, 0, false, 256>(P, st);   // kpad0 <= DVD_MLP_MAX_NIN (check_cfg_supported)
   }
-  DVD_CUDA_LAUNCH_CHECK("mlp_dgrad");
-  return 0;
 }
 
 extern "C" int dvd_mlp_wgrad(const dvd_mlp_cfg* cfg, const void* save_e, const void* dy_scratch, float* const* g_w,
@@ -836,7 +911,8 @@ extern "C" int dvd_mlp_wgrad(const dvd_mlp_cfg* cfg, const void* save_e, const v
         J.out = g_w[5]; J.ld = kWidth; J.transposed = 1; J.m_off = mh * 128; J.m_valid = kWidth; J.n_valid = 3;
         J.bias_out = nullptr;
       }
-      DVD_ARG_CHECK(J.n == 256 || J.n == 144 || J.n == 112 || J.n == 16, "no weight-gradient kernel for a %d-channel operand", J.n);
+      DVD_ARG_CHECK(J.n == 256 || J.n == 192 || J.n == 144 || J.n == 128 || J.n == 112 || J.n == 64 || J.n == 16,
+                    "no weight-gradient kernel for a %d-channel operand", J.n);
     }
   }
   int ksplit = num_sms() / nj;

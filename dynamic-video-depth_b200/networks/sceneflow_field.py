@@ -16,6 +16,7 @@ class SceneFlowFieldNet(nn.Module):
             raise NotImplementedError(
                 'dvd_b200 implements the configuration the reference Model instantiates '
                 '(net_width=256, n_layers=4, lrelu, no norm; models/scene_flow_motion_field.py:107)')
+        ops.check_mlp_counts(N_freq_xyz, N_freq_t, time_dependent)   # fail at construction, not at the first step
         n_xyz = 3 + 6 * N_freq_xyz
         n_t = 1 + 2 * N_freq_t
         n_in = n_xyz + n_t if time_dependent else n_xyz

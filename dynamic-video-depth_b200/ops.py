@@ -216,18 +216,37 @@ def reproject_loss(depth_1, depth_2, sf, flow, mask, poses, cfg, gscale=1.0):
 # ================================================================================================
 # scene-flow MLP (wgmma kernels)
 
+def mlp_n_in(n_freq_xyz, n_freq_t, time_dependent):
+    """Input width of the scene-flow MLP's first layer (networks/sceneflow_field.py:22-24)."""
+    return (1 + 2 * n_freq_t if time_dependent else 0) + 3 + 6 * n_freq_xyz
+
+
+def check_mlp_counts(n_freq_xyz, n_freq_t, time_dependent):
+    """Raise ValueError unless the kernels run this positional encoding: non-negative counts and at most
+    DVD_MLP_MAX_NIN (256) input features (n_freq_t is ignored when the field is not time-dependent)."""
+    if int(n_freq_xyz) != n_freq_xyz or int(n_freq_t) != n_freq_t or n_freq_xyz < 0 or (time_dependent and n_freq_t < 0):
+        raise ValueError('n_freq_xyz / n_freq_t must be non-negative integers (got %r, %r)' % (n_freq_xyz, n_freq_t))
+    nin = mlp_n_in(n_freq_xyz, n_freq_t, time_dependent)
+    if nin > _lib.DVD_MLP_MAX_NIN:
+        raise ValueError('scene-flow MLP input width (time_dependent ? 1 + 2 n_freq_t : 0) + 3 + 6 n_freq_xyz = %d for '
+                         'n_freq_xyz=%d n_freq_t=%d time_dependent=%s exceeds the supported %d'
+                         % (nin, n_freq_xyz, n_freq_t, bool(time_dependent), _lib.DVD_MLP_MAX_NIN))
+
+
 def make_mlp_cfg(n_freq_xyz=16, n_freq_t=16, time_dependent=True, sf_mag_div=100.0):
     """struct dvd_mlp_cfg; frequencies = torch.linspace(1, N+1, N) in fp32 exactly as
-    PeriodicEmbed builds them (networks/blocks.py:23-24)."""
-    if n_freq_xyz > 16 or n_freq_t > 16:
-        raise ValueError('n_freq_xyz / n_freq_t must be <= 16')
+    PeriodicEmbed builds them (networks/blocks.py:23-24). Any encoding with at most 256 input features
+    (check_mlp_counts)."""
+    check_mlp_counts(n_freq_xyz, n_freq_t, time_dependent)
     c = MlpCfg()
     c.n_freq_xyz, c.n_freq_t, c.time_dependent, c.sf_mag_div = int(n_freq_xyz), int(n_freq_t), int(bool(time_dependent)), float(sf_mag_div)
+    n_t = int(n_freq_t) if time_dependent else 0
     fx = torch.linspace(1, n_freq_xyz + 1, steps=n_freq_xyz, dtype=torch.float32).tolist() if n_freq_xyz > 0 else []
-    ft = torch.linspace(1, n_freq_t + 1, steps=n_freq_t, dtype=torch.float32).tolist() if n_freq_t > 0 else []
-    for i in range(16):
-        c.freq_xyz[i] = fx[i] if i < len(fx) else 0.0
-        c.freq_t[i] = ft[i] if i < len(ft) else 0.0
+    ft = torch.linspace(1, n_t + 1, steps=n_t, dtype=torch.float32).tolist() if n_t > 0 else []
+    for i, f in enumerate(fx):
+        c.freq_xyz[i] = f
+    for i, f in enumerate(ft):
+        c.freq_t[i] = f
     return c
 
 

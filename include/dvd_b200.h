@@ -117,14 +117,22 @@ int dvd_selftest_umma(const float* A, const float* B, float* D, int K, int N, in
  * All GEMMs run on wgmma tensor cores with fp32 emulated as two bf16 planes (x = hi + lo,
  * D += Ahi*Bhi + Alo*Bhi + Ahi*Blo, fp32 accumulate): error ~2e-5, i.e. tighter than the
  * TF32 path the reference itself takes on a GPU (cudnn.allow_tf32 default).
- * Fixed by the reference ctor (smf.py:107): width 256, 4 hidden layers, 3 outputs.             */
+ * Fixed by the reference ctor (smf.py:107): width 256, 4 hidden layers, 3 outputs. The positional encoding
+ * follows --n_freq_xyz, --n_freq_t and --time_dependent (networks/sceneflow_field.py:22-35): the first layer
+ * reads nin = (time_dependent ? 1 + 2 n_freq_t : 0) + 3 + 6 n_freq_xyz features, and every configuration
+ * with nin <= DVD_MLP_MAX_NIN runs (a count of 0 is the reference's nn.Identity). (16, 16, time-dependent)
+ * and (16, time-independent) have kernels compiled for their counts; every other one runs the generic kernels,
+ * whose first layer is padded to a multiple of 64 input channels. Larger configurations return -2.          */
+#define DVD_MLP_MAX_NIN 256
+#define DVD_MLP_MAX_FREQ_XYZ 42   /* (DVD_MLP_MAX_NIN - 3) / 6 */
+#define DVD_MLP_MAX_FREQ_T 126    /* (DVD_MLP_MAX_NIN - 4) / 2 */
 typedef struct dvd_mlp_cfg {
   int   n_freq_xyz;      /* --n_freq_xyz (16) */
-  int   n_freq_t;        /* --n_freq_t   (16) */
+  int   n_freq_t;        /* --n_freq_t   (16); ignored unless time_dependent */
   int   time_dependent;  /* --time_dependent */
   float sf_mag_div;      /* --sf_mag_div (100) */
-  float freq_xyz[16];    /* torch.linspace(1, n_freq+1, n_freq) in fp32 (networks/blocks.py:23-24) */
-  float freq_t[16];
+  float freq_xyz[DVD_MLP_MAX_FREQ_XYZ];  /* torch.linspace(1, n_freq+1, n_freq) in fp32 (networks/blocks.py:23-24) */
+  float freq_t[DVD_MLP_MAX_FREQ_T];
 } dvd_mlp_cfg;
 
 /* sizes (bytes) of the caller-allocated scratch buffers for a given configuration */
