@@ -105,7 +105,11 @@ SIGNATURES = {
                        ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float), _P, _I, _I, _I, _P],
     'dvd_head_fwd': [_P, _P, _P, _P, ctypes.c_long, _P],
     'dvd_head_bwd': [_P, _P, _P, _P, _P, _P, _P, ctypes.c_long, _I, _I, _P],
+    'dvd_flow_resize_cubic': [_P, ctypes.c_size_t, _P, ctypes.c_size_t, _I, _I, _I, _I, _I, _P],
+    'dvd_flow_pair_masks': [_P, _P, ctypes.c_size_t, _P, _P, ctypes.c_size_t, _I, _I, _I, _I, _P],
 }
+DVD_MASKS_FLOWPAIR_U8 = 0
+DVD_MASKS_PAIRFILE_F32 = 1
 _RESTYPES = {'dvd_last_error': ctypes.c_char_p, 'dvd_struct_size': ctypes.c_long, 'dvd_conv2d_workspace_bytes': ctypes.c_size_t, 'dvd_conv2d_pack_blocks': ctypes.c_long, 'dvd_mlp_packed_weights_bytes': ctypes.c_size_t,
              'dvd_mlp_save_bytes_per_eval': ctypes.c_size_t, 'dvd_mlp_dy_bytes': ctypes.c_size_t}
 

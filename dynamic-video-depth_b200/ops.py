@@ -573,3 +573,57 @@ def reproject_tensors(depth_1, depth_2, sf, flow, poses):
     """dict of the nine differentiable per-pixel tensors."""
     _chk_reproject(depth_1.contiguous(), depth_2.contiguous(), flow, None, sf.contiguous() if sf is not None else None, poses)
     return dict(zip(_MAT_ALL, ReprojectMaterialize.apply(depth_1, depth_2, sf, flow, poses)))
+
+
+# ---- flow-pair preprocessing (csrc/flow_pairs.cu) ---------------------------------------------------------------------------
+MASK_CONVENTIONS = {'flowpair': _lib.DVD_MASKS_FLOWPAIR_U8, 'pair_file': _lib.DVD_MASKS_PAIRFILE_F32}
+
+
+def _chk_flows(flow, name):
+    _chk(flow, name)
+    if flow.dim() != 4 or flow.shape[-1] != 2:
+        raise ValueError('%s must be [B,H,W,2] (NHWC flow), got %s' % (name, tuple(flow.shape)))
+    if flow.data_ptr() % 8:
+        raise ValueError('%s must be 8-byte aligned' % name)
+    return flow
+
+
+def flow_resize_cubic(flow, H, W):
+    """The reference's `resize_flow` (generate_flows.py:44-54) on the GPU: cv2 INTER_CUBIC resize of [B,h,w,2] fp32 flows to
+    [B,H,W,2], then x *= W / w and y *= H / h."""
+    _chk_flows(flow, 'flow')
+    H, W = int(H), int(W)
+    if H < 1 or W < 1:
+        raise ValueError('output size must be positive, got %dx%d' % (H, W))
+    B, h, w, _ = flow.shape
+    out = torch.empty(B, H, W, 2, dtype=torch.float32, device=flow.device)
+    lib = _lib.load()
+    LAUNCHES['n'] += 1
+    _lib.check(lib.dvd_flow_resize_cubic(_ptr(flow), flow.numel() * 4, _ptr(out), out.numel() * 4, B, h, w, H, W, _stream()),
+               'dvd_flow_resize_cubic')
+    return out
+
+
+def flow_pair_masks(flow_1_2, flow_2_1, convention='pair_file'):
+    """Forward / backward consistency masks of two [B,H,W,2] fp32 flows (generate_flows.py:57-82,139-148) -> (mask_1, mask_2).
+    convention 'flowpair': uint8 [B,H,W], 1 = inconsistent or out of bounds (flowpair_*.npz);
+               'pair_file': fp32 [B,H,W,1,1], 1 - ceil(mask), 1 = valid (the sequence .pt files, the Model's mask_1 / mask_2)."""
+    if convention not in MASK_CONVENTIONS:
+        raise ValueError('convention must be one of %s, got %r' % (sorted(MASK_CONVENTIONS), convention))
+    _chk_flows(flow_1_2, 'flow_1_2')
+    _chk_flows(flow_2_1, 'flow_2_1')
+    if flow_1_2.shape != flow_2_1.shape or flow_1_2.device != flow_2_1.device:
+        raise ValueError('flow_1_2 %s and flow_2_1 %s must match' % (tuple(flow_1_2.shape), tuple(flow_2_1.shape)))
+    B, H, W, _ = flow_1_2.shape
+    if H < 2 or W < 2:
+        raise ValueError('flows must be at least 2x2, got %dx%d' % (H, W))
+    u8 = convention == 'flowpair'
+    shape, dtype = ((B, H, W), torch.uint8) if u8 else ((B, H, W, 1, 1), torch.float32)
+    m1 = torch.empty(shape, dtype=dtype, device=flow_1_2.device)
+    m2 = torch.empty_like(m1)
+    lib = _lib.load()
+    LAUNCHES['n'] += 1
+    _lib.check(lib.dvd_flow_pair_masks(_ptr(flow_1_2), _ptr(flow_2_1), flow_1_2.numel() * 4, _ptr(m1), _ptr(m2),
+                                       m1.numel() * m1.element_size(), B, H, W, MASK_CONVENTIONS[convention], _stream()),
+               'dvd_flow_pair_masks')
+    return m1, m2

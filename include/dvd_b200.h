@@ -318,6 +318,21 @@ int dvd_head_fwd(const float* x, const float* w, const float* b, float* depth, l
 int dvd_head_bwd(const float* x, const float* w, const float* b, const float* g_depth, float* gx, float* gw, float* gb, long P,
                  int relu_mask, int round_out, void* stream);
 
+/* ---- flow-pair preprocessing (csrc/flow_pairs.cu): raw optical flows -> the training pair's flows and masks ------------------
+ * scripts/preprocess/davis/generate_flows.py:44-82,139-148. Flows are NHWC fp32 [B,H,W,2] (the pair-file layout), 8-byte
+ * aligned; every call checks its shapes, alignment and buffer byte sizes before it launches and returns -2 with a message.   */
+/* resize_flow: cv2.resize(flow, (W, H), INTER_CUBIC) (half-pixel centres, A = -0.75, clamped taps, horizontal pass first), then
+ * x *= W / w and y *= H / h. src [B,h,w,2] -> dst [B,H,W,2], any sizes.                                                      */
+int dvd_flow_resize_cubic(const float* src, size_t src_bytes, float* dst, size_t dst_bytes, int B, int h, int w, int H, int W,
+                          void* stream);
+/* forward / backward consistency masks. mask_1 lives on frame 2's grid: q = p + flow_2_1(p); flow_1_2 sampled at q as
+ * F.grid_sample does (bilinear, zeros padding, align_corners=True); the pixel is bad when |sample + flow_2_1(p)| > 1 or q lies
+ * outside [0, W-1] x [0, H-1]. mask_2 is the same with the flows swapped. Output convention:                               */
+#define DVD_MASKS_FLOWPAIR_U8 0    /* uint8 [B,H,W], 1 = bad (flowpair_*.npz)                                               */
+#define DVD_MASKS_PAIRFILE_F32 1   /* fp32 [B,H,W,1,1], 1 - ceil(mask): 1 = valid (the sequence .pt files); 4-byte aligned  */
+int dvd_flow_pair_masks(const float* flow_1_2, const float* flow_2_1, size_t flow_bytes, void* mask_1, void* mask_2,
+                        size_t mask_bytes, int B, int H, int W, int convention, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
