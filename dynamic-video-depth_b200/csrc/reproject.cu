@@ -683,6 +683,9 @@ __device__ __forceinline__ bool staged_pairs(const float* __restrict__ depth_1, 
     const float2 sy = *reinterpret_cast<const float2*>(src + 3 * kTile);
     const float2 sz = *reinterpret_cast<const float2*>(src + 4 * kTile);
     const float4 f = *reinterpret_cast<const float4*>(src + 5 * kTile + tv);
+    // The producer's next bulk copy into this stage is an async-proxy write: without a proxy fence the generic-proxy
+    // loads above are not ordered before it, and a few lanes read the next tile's bytes (seen as wrong g_sf on H100).
+    fence_proxy_async_smem();
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[s]);     // values are in registers: hand the stage back
     const int bl = tile / tiles_per_pair, p = (tile - bl * tiles_per_pair) * kTile + tv;
