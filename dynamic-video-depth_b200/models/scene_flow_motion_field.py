@@ -296,6 +296,9 @@ class Model(NetInterface):
             dev_logs, d1, d2, sf, poses = self._step_body(self._input, steps, dt)
             logs = dev_logs.cpu()    # ONE device->host read per step
             vis = (d1, d2, sf, poses)
+        # the Adam step wrote the MLP weights through a raw pointer (no version bump, same address): the cached wgmma pack of
+        # the eval forward (`_predict_on_batch`) is stale on both branches - captured graphs re-pack inside `_step_body`
+        self.net_sceneflow._packed_version = None
         # `**loss_data` overrides the step-weighted 'loss' in the reference's dict literal (smf.py:226,321)
         has_reg = o.interp_steps > 0 and (not self.warm or o.warm_reg) and o.acc_mul > 0
         batch_log = {'size': o.batch_size, 'loss': float(logs[3]), 'total_loss': float(logs[3]),
