@@ -107,6 +107,8 @@ SIGNATURES = {
     'dvd_head_bwd': [_P, _P, _P, _P, _P, _P, _P, ctypes.c_long, _I, _I, _P],
     'dvd_flow_resize_cubic': [_P, ctypes.c_size_t, _P, ctypes.c_size_t, _I, _I, _I, _I, _I, _P],
     'dvd_flow_pair_masks': [_P, _P, ctypes.c_size_t, _P, _P, ctypes.c_size_t, _I, _I, _I, _I, _P],
+    'dvd_disp_vali_partials_size': [_I, _I, _I],
+    'dvd_disp_vali': [_P, _P, _P, _P, _P, _I, _I, _I, _P],
 }
 DVD_MASKS_FLOWPAIR_U8 = 0
 DVD_MASKS_PAIRFILE_F32 = 1

@@ -459,8 +459,70 @@ class Model(NetInterface):
         gt = batch['depth_mvs'].to(pred['depth'].device)
         return {'size': batch['img'].shape[0], 'loss': self.disp_vali(pred['depth'], gt).item()}
 
+    def validate_sequence(self, frames, batch_size=1, chunk=8):
+        """The reference's validation pass (train.py:234,319-346 with `_vali_on_batch`) over a device-resident sequence.
+
+        `frames` holds the `vali` items of the dataset stacked along dim 0 (at least 'img' [F,3,H,W] and 'depth_mvs'
+        [F,1,H,W], on the model's device). Batches of `batch_size` frames are formed as the reference's loader does
+        (drop_last=True). Depth runs `chunk` frames at a time through the inference forward of the depth net (no saved
+        activations), and `dvd_disp_vali` writes each frame's squared-error sum into one device buffer that is read back once.
+
+        Returns the reference's `loss_eval`: the size-weighted mean of the per-batch `disp_vali` losses, i.e. the mean per-frame
+        MSE over the frames of the complete batches. The step graphs, the MLP's wgmma pack and the nets' train / eval modes are
+        left as they were."""
+        img, gt = frames['img'], frames['depth_mvs']
+        n = (img.shape[0] // batch_size) * batch_size
+        if n < 1:
+            raise ValueError('validate_sequence needs at least one batch of %d frames, got %d' % (batch_size, img.shape[0]))
+        if img.device != self.device or gt.device != self.device:
+            raise ValueError('validate_sequence expects the frames on %s (move the sequence to the device once)' % self.device)
+        H, W = gt.shape[-2:]
+        modes = [net.training for net in self._nets]
+        for net in self._nets:
+            net.eval()
+        sse = torch.empty(n, dtype=torch.float32, device=self.device)
+        try:
+            with torch.no_grad():
+                for s in range(0, n, chunk):
+                    e = min(s + chunk, n)
+                    x = img[s:e]
+                    depth = self.net_depth(x) if self.opt.midas else self.net_depth(x, None)
+                    ops.disp_vali(depth.contiguous(), gt[s:e].float().contiguous(), out=sse[s:e])
+        finally:
+            for net, m in zip(self._nets, modes):
+                net.train(m)
+        per_frame = sse.cpu().double() / float(H * W)      # the one read-back of the pass
+        batch_losses = per_frame.reshape(-1, batch_size).mean(1)
+        return float(batch_losses.mean())
+
+    def pack_output(self, pred_all, batch):
+        """video_base.py:105-126 for the per-frame (`img`) batches of the test pass."""
+        out = {'batch_size': len(batch['pair_path']), 'img_1': batch['img'].cpu().numpy(), 'img_2': batch['img'].cpu().numpy()}
+        out.update(pred_all)
+        out['depth_nn'] = batch['depth_pred'].cpu().numpy()
+        out['depth_gt'] = batch['depth_mvs'].cpu().numpy()
+        out['cam_c2w'] = batch['cam_c2w'].cpu().numpy()
+        out['K'] = batch['K'].cpu().numpy()
+        out['pair_path'] = batch['pair_path']
+        return out
+
     def test_on_batch(self, batch_idx, batch):
+        """Refined depth and scene flow of one per-frame batch. With `opt.output_dir` set (the test driver sets it), also writes
+        <output_dir>/epoch{best|%04d}_test/batch%04d.npz with the reference's `pack_output` keys (video_base.py:128-155)."""
         self.eval()
         self.load_batch(batch)
         pred = self._predict_on_batch(is_train=False)
-        return {k: v.cpu().numpy() for k, v in pred.items()}
+        pred = {k: v.cpu().numpy() for k, v in pred.items()}
+        out_root = getattr(self.opt, 'output_dir', None)
+        if out_root:
+            epoch_string = 'best' if self.opt.epoch < 0 else '%04d' % self.opt.epoch
+            outdir = join(out_root, 'epoch%s_test' % epoch_string)
+            makedirs(outdir, exist_ok=True)
+            output = self.pack_output({k: v.copy() for k, v in pred.items()}, batch)
+            if batch_idx == 223:
+                # kept on purpose: the reference overwrites the first two depth rows of batch 223 with the third
+                # (video_base.py:148-150), so exported files stay interchangeable with its own
+                output['depth'][0, 0, 0, :] = output['depth'][0, 0, 2, :]
+                output['depth'][0, 0, 1, :] = output['depth'][0, 0, 2, :]
+            np.savez(join(outdir, 'batch%04d' % batch_idx), **output)
+        return pred

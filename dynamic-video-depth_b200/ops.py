@@ -627,3 +627,32 @@ def flow_pair_masks(flow_1_2, flow_2_1, convention='pair_file'):
                                        m1.numel() * m1.element_size(), B, H, W, MASK_CONVENTIONS[convention], _stream()),
                'dvd_flow_pair_masks')
     return m1, m2
+
+
+# ---- validation metric (csrc/eval_ops.cu) -----------------------------------------------------------------------------------
+def disp_vali(depth, depth_gt, want_terms=False, out=None):
+    """The reference's `disp_vali` (models/video_base.py:66-74) per frame: depth, depth_gt [N,1,H,W] fp32 -> frame_sse [N], the
+    sum over each frame of (disp(depth)·v - disp(gt)·v)² with v = [gt > 1e-2] (bitwise torch's fp32 terms, fixed-order sums).
+    A frame's MSE is frame_sse / (H·W). `out` may be a caller-owned contiguous [N] fp32 buffer (e.g. a slice of a longer one).
+    With want_terms, returns (frame_sse, terms [N,1,H,W])."""
+    _chk(depth, 'depth')
+    _chk(depth_gt, 'depth_gt')
+    if depth.dim() != 4 or depth.shape[1] != 1:
+        raise ValueError('depth must be [N,1,H,W], got %s' % (tuple(depth.shape),))
+    if depth_gt.shape != depth.shape or depth_gt.device != depth.device:
+        raise ValueError('depth_gt %s must match depth %s' % (tuple(depth_gt.shape), tuple(depth.shape)))
+    N, _, H, W = depth.shape
+    if out is None:
+        out = torch.empty(N, dtype=torch.float32, device=depth.device)
+    else:
+        _chk(out, 'out', (N,))
+    terms = torch.empty_like(depth) if want_terms else None
+    lib = _lib.load()
+    n_part = lib.dvd_disp_vali_partials_size(N, H, W)
+    if n_part < 1:
+        raise ValueError('bad shape for dvd_disp_vali: %s' % (tuple(depth.shape),))
+    partials = torch.empty(n_part, dtype=torch.float32, device=depth.device)
+    LAUNCHES['n'] += 2
+    _lib.check(lib.dvd_disp_vali(_ptr(depth), _ptr(depth_gt), _ptr(out), _ptr(terms), _ptr(partials), N, H, W, _stream()),
+               'dvd_disp_vali')
+    return (out, terms) if want_terms else out

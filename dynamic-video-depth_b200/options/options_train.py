@@ -65,6 +65,9 @@ def add_general_arguments(parser):
     a('--resident', action='store_true', help='keep the whole sequence on the GPU and draw gap-bucketed, rank-disjoint batches '
                                               '(datasets/resident.py) instead of one pair file per step through a DataLoader')
     a('--pairs_per_step', type=int, default=1, help='frame pairs per step and GPU with --resident (the reference ships 1 per file)')
+    a('--validate', action='store_true', help='validate after every epoch (and before the first with --vali_at_start) on the '
+                                              "dataset's vali frames, at most --vali_batches batches, log loss_eval and keep "
+                                              'best.pt at the lowest loss_eval (train.py:150-166,319-346 of the reference)')
     return parser, unique_params
 
 

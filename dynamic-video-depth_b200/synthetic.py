@@ -98,6 +98,26 @@ def make_batch(pairs, H=224, W=384, n_frames=80, seed=0, smooth_flow=False, dtyp
     return out
 
 
+def make_frame(idx, H=224, W=384, n_frames=80, invalid_p=0.1):
+    """One per-frame `vali` item of frame `idx` with the keys and layouts of datasets/davis_sequence.py:117-152 (pose tensors
+    hold transposes as in make_batch; cam_c2w is the 4x4 camera-to-world matrix). `depth_mvs` is a seeded smooth depth map in
+    [2, 8] with a share `invalid_p` of its pixels set to 0 (invalid); `depth_pred` another one in [1.5, 9]."""
+    g = torch.Generator().manual_seed(100003 + idx)
+    R, t, K = camera(idx, H, W)
+    c2w = torch.eye(4, dtype=torch.float64)
+    c2w[:3, :3], c2w[:3, 3] = R, t
+    gt = make_depths(1, H, W, seed=200003 + idx)[0]
+    gt = gt * (torch.rand(1, H, W, generator=g, dtype=torch.float64) >= invalid_p).float()
+    s = {'time_stamp_1': torch.full((1, H, W), idx / n_frames, dtype=torch.float64),
+         'img': torch.rand(3, H, W, generator=g, dtype=torch.float64), 'frame_id_1': idx, 'time_step': 1.0 / n_frames,
+         'depth_pred': make_depths(1, H, W, seed=300003 + idx, lo=1.5, hi=9.0)[0], 'cam_c2w': c2w, 'depth_mvs': gt,
+         'R_1': R.t().reshape(1, 1, 3, 3), 'R_1_T': R.reshape(1, 1, 3, 3), 't_1': t.reshape(1, 1, 1, 3),
+         'K': K.t().reshape(1, 1, 3, 3), 'K_inv': torch.linalg.inv(K).t().reshape(1, 1, 3, 3)}
+    s = {k: (v.float().contiguous() if torch.is_tensor(v) else v) for k, v in s.items()}
+    s['pair_path'] = 'synthetic_frame_%03d' % idx
+    return s
+
+
 def make_depths(B, H, W, seed=1, lo=2.0, hi=8.0, dtype=torch.float32):
     """Smooth positive depth maps for op-level tests (the depth nets are tested separately)."""
     g = torch.Generator().manual_seed(seed)

@@ -18,6 +18,54 @@ from .models.netinterface import NullLogger
 from .options import options_train
 
 
+def stack_frames(dataset, n, device):
+    """The first `n` items of a per-frame (`vali`) dataset as one batch dict (what a DataLoader with batch_size=n yields), its
+    tensors moved to `device` once."""
+    batch = torch.utils.data.default_collate([dataset[i] for i in range(n)])
+    return {k: (v.to(device) if torch.is_tensor(v) else v) for k, v in batch.items()}
+
+
+class _Validator:
+    """--validate: the reference's per-epoch validation (train.py:234,319-346) and its best-model rule (ModelSaveLogger with
+    save_best, loggers/loggers.py:259-306; train.py:150-166): best.pt is written, with the optimizers, whenever loss_eval is
+    strictly lower than the best so far, which on resume is read from the existing best.pt."""
+
+    def __init__(self, opt, model, Dataset, device):
+        self.opt, self.model = opt, model
+        ds = Dataset(opt, mode='vali', model=model)
+        bs = max(1, opt.batch_size)
+        n = len(ds) if opt.vali_batches is None else min(len(ds), opt.vali_batches * bs)
+        n = (n // bs) * bs                       # the reference's vali loader drops the last incomplete batch
+        if n < 1:
+            raise SystemExit('--validate: the vali set has %d frames, fewer than one batch of --batch_size %d' % (len(ds), bs))
+        self.batch_size = bs
+        self.frames = stack_frames(ds, n, device)
+        self.best_path = os.path.join(opt.full_logdir, 'best.pt') if opt.full_logdir else None
+        self.best = None
+        if opt.resume != 0 and self.best_path and os.path.isfile(self.best_path):
+            self.best = torch.load(self.best_path, map_location='cpu', weights_only=False).get('loss_eval')
+        self.loss_eval = {}
+
+    def __call__(self, epoch):
+        v = self.model.validate_sequence(self.frames, batch_size=self.batch_size)
+        self.loss_eval[epoch] = v
+        if self.best_path and (self.best is None or v < self.best):
+            self.best = v
+            self.model.save_state_dict(self.best_path, save_optimizer=True, additional_values={'epoch': epoch, 'loss_eval': v})
+
+
+def save_opt(opt):
+    """opt.pt (the options as a dict, what the reference's test.py loads) and opt.txt in the log directory (train.py:88-96)."""
+    logdir = opt.full_logdir
+    if os.path.exists(os.path.join(logdir, 'opt.pt')) and opt.pt_no_overwrite:
+        return
+    os.makedirs(logdir, exist_ok=True)
+    torch.save(vars(opt), os.path.join(logdir, 'opt.pt'))
+    with open(os.path.join(logdir, 'opt.txt'), 'w') as fout:
+        for k, v in vars(opt).items():
+            fout.write('%20s\t%-20s\n' % (k, v))
+
+
 def main_worker(local_rank, ngpus, opt):
     env_world = int(os.environ.get('WORLD_SIZE', '1'))
     distributed = opt.multiprocess_distributed or env_world > 1
@@ -71,6 +119,8 @@ def main_worker(local_rank, ngpus, opt):
         loader = torch.utils.data.DataLoader(ds, batch_size=1, shuffle=sampler is None, sampler=sampler,
                                              num_workers=opt.workers, pin_memory=True, drop_last=True)
 
+    validator = _Validator(opt, model, Dataset, device) if (opt.validate and rank == 0) else None
+
     def on_epoch(epoch):
         if sampler is not None:
             sampler.set_epoch(epoch)
@@ -80,11 +130,23 @@ def main_worker(local_rank, ngpus, opt):
                                   additional_values={'epoch': epoch})
             model.save_state_dict(os.path.join(opt.full_logdir, 'checkpoint.pt'), save_optimizer=True,
                                   additional_values={'epoch': epoch})
+        if validator is not None:
+            validator(epoch)
+    if validator is not None and opt.vali_at_start:
+        validator(initial_epoch - 1)
     model.train_epoch(loader, epochs=opt.epoch, initial_epoch=initial_epoch, max_batches_per_train=opt.epoch_batches,
                       global_rank=rank, train_epoch_callback=on_epoch)
-    if rank == 0:
+    if rank == 0 and validator is None:
         for e, log in logger.epoch_logs:
             print('epoch %d:' % e, {k: round(v, 6) for k, v in log.items()})
+    elif rank == 0:
+        # the validation of epoch e joins that epoch's training log; --vali_at_start adds epoch initial_epoch - 1
+        logs = dict(logger.epoch_logs)
+        for e in sorted(set(logs) | set(validator.loss_eval)):
+            log = {k: round(v, 6) for k, v in logs.get(e, {}).items()}
+            if e in validator.loss_eval:
+                log['loss_eval'] = validator.loss_eval[e]     # unrounded: it is the value best.pt records
+            print('epoch %d:' % e, log)
     if distributed:
         model.release_graphs()
         dist.destroy_process_group()
@@ -94,6 +156,8 @@ def main(argv=None):
     opt, _ = options_train.parse(argv)
     if opt.full_logdir is None and opt.logdir:
         opt.full_logdir = os.path.join(opt.logdir, '%s_%s' % (opt.net, opt.dataset), str(opt.expr_id))
+    if opt.full_logdir and int(os.environ.get('RANK', '0')) == 0:
+        save_opt(opt)
     ngpus = max(1, len([g for g in str(opt.gpu).split(',') if g not in ('none', '')]))
     if opt.multiprocess_distributed and int(os.environ.get('WORLD_SIZE', '1')) == 1:
         mp.spawn(main_worker, nprocs=ngpus, args=(ngpus, opt))

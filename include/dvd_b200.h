@@ -333,6 +333,18 @@ int dvd_flow_resize_cubic(const float* src, size_t src_bytes, float* dst, size_t
 int dvd_flow_pair_masks(const float* flow_1_2, const float* flow_2_1, size_t flow_bytes, void* mask_1, void* mask_2,
                         size_t mask_bytes, int B, int H, int W, int convention, void* stream);
 
+/* ---- validation metric (csrc/eval_ops.cu) ----------------------------------------------------------------------------------
+ * disp_vali (models/video_base.py:66-74) per frame: depth, depth_gt [N,1,H,W] fp32 (4-byte aligned; 16-byte aligned with H*W a
+ * multiple of 4 takes the vector path). With v = [gt > 1e-2] and disp(x) = (1 / (x + (1 - [x > 1e-2])·1e-8))·[x > 1e-2], the
+ * per-pixel term t = (disp(depth)·v - disp(gt)·v)² is evaluated in torch's operation order with every operation rounded on its
+ * own, so it equals torch's fp32 elementwise term bit for bit. frame_sse [N] = Σ t over each frame, summed in a fixed order
+ * without atomics (block partials into `partials`, then one fixed-order pass): bitwise reproducible. The frame's MSE is
+ * frame_sse / (H·W). terms [N,1,H,W] receives the per-pixel terms, or is NULL. `partials` holds
+ * dvd_disp_vali_partials_size(N, H, W) floats (-1 for a bad shape). Returns -2 with a message on a shape / alignment error.   */
+int dvd_disp_vali_partials_size(int N, int H, int W);
+int dvd_disp_vali(const float* depth, const float* depth_gt, float* frame_sse, float* terms, float* partials, int N, int H, int W,
+                  void* stream);
+
 #ifdef __cplusplus
 }
 #endif
