@@ -109,11 +109,26 @@ SIGNATURES = {
     'dvd_flow_pair_masks': [_P, _P, ctypes.c_size_t, _P, _P, ctypes.c_size_t, _I, _I, _I, _I, _P],
     'dvd_disp_vali_partials_size': [_I, _I, _I],
     'dvd_disp_vali': [_P, _P, _P, _P, _P, _I, _I, _I, _P],
+    'dvd_raft_stem_fwd': [_P, _P, _P, _P, ctypes.c_size_t, _I, _I, _I, _P],
+    'dvd_raft_instnorm_scratch_bytes': [_I, _I],
+    'dvd_raft_instnorm_stats': [_P, _P, _P, ctypes.c_size_t, _I, ctypes.c_long, _I, _F, _P],
+    'dvd_raft_norm_act': [_P, _P, _P, _P, _I, ctypes.c_long, _I, _I, _I, _I, _P],
+    'dvd_raft_pyramid_floats': [_I, _I, _I],
+    'dvd_raft_corr_pyramid': [_P, _P, _P, ctypes.c_size_t, _I, _I, _I, _I, _P],
+    'dvd_raft_lookup': [_P, ctypes.c_size_t, _P, _P, ctypes.c_size_t, _I, _I, _I, _I, _P],
+    'dvd_raft_convf1': [_P, _P, _P, _P, _I, _I, _I, _I, _P],
+    'dvd_raft_context_split': [_P, _P, _P, _P, ctypes.c_long, _P],
+    'dvd_raft_motion_pack': [_P, _P, _P, _P, _I, _I, _I, _P],
+    'dvd_raft_gru_rh': [_P, _P, _P, ctypes.c_long, _P],
+    'dvd_raft_gru_update': [_P, _P, _P, _P, _P, ctypes.c_long, _P],
+    'dvd_raft_flow_head': [_P, _P, _P, _P, _P, _I, _I, _I, _P],
+    'dvd_raft_upsample': [_P, _P, _P, _P, _P, ctypes.c_size_t, _I, _I, _I, _F, _P],
 }
 DVD_MASKS_FLOWPAIR_U8 = 0
 DVD_MASKS_PAIRFILE_F32 = 1
 _RESTYPES = {'dvd_last_error': ctypes.c_char_p, 'dvd_struct_size': ctypes.c_long, 'dvd_conv2d_workspace_bytes': ctypes.c_size_t, 'dvd_conv2d_pack_blocks': ctypes.c_long, 'dvd_mlp_packed_weights_bytes': ctypes.c_size_t,
-             'dvd_mlp_save_bytes_per_eval': ctypes.c_size_t, 'dvd_mlp_dy_bytes': ctypes.c_size_t}
+             'dvd_mlp_save_bytes_per_eval': ctypes.c_size_t, 'dvd_mlp_dy_bytes': ctypes.c_size_t,
+             'dvd_raft_instnorm_scratch_bytes': ctypes.c_long, 'dvd_raft_pyramid_floats': ctypes.c_long}
 
 _lib = None
 

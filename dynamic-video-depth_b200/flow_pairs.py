@@ -70,22 +70,55 @@ def to_dataset_item(pf, n_frames, unit=1.0):
 def process_raw_flows(flow_1_2, flow_2_1, H, W, device=None):
     """raw flows [B,h,w,2] (host arrays or tensors, one gap) -> host tensors (flow_1_2, flow_2_1 [B,H,W,2] fp32, mask_1,
     mask_2 [B,H,W] uint8, 1 = bad): one resize launch per direction when (h, w) != (H, W), then one mask launch."""
-    from . import ops
     device = torch.device(device if device is not None else 'cuda')
     if device.type != 'cuda':
         raise RuntimeError('raw flows are resized and masked by the CUDA kernels of dvd_b200; a CUDA device is needed')
     f12 = torch.as_tensor(flow_1_2, dtype=torch.float32).to(device, non_blocking=True).contiguous()
     f21 = torch.as_tensor(flow_2_1, dtype=torch.float32).to(device, non_blocking=True).contiguous()
+    return tuple(t.cpu() for t in finish_flows(f12, f21, H, W))
+
+
+def finish_flows(f12, f21, H, W):
+    """device flows [B,h,w,2] -> (flow_1_2, flow_2_1 [B,H,W,2], mask_1, mask_2 [B,H,W] uint8), still on the device"""
+    from . import ops
     if tuple(f12.shape[1:3]) != (H, W):
         f12, f21 = ops.flow_resize_cubic(f12, H, W), ops.flow_resize_cubic(f21, H, W)
     m1, m2 = ops.flow_pair_masks(f12, f21, convention='flowpair')
-    return tuple(t.cpu() for t in (f12, f21, m1, m2))
+    return f12, f21, m1, m2
+
+
+RAFT_SIZE = (288, 512)      # generate_flows.py:121-122
+
+
+def raft_images(frames, size=RAFT_SIZE):
+    """The frames' colour images at RAFT's resolution, [n,3,h,w] fp32 in 0..255 (generate_flows.py:119-126). The reference
+    resizes with skimage.transform.resize(anti_aliasing=True); this is cv2.resize with INTER_AREA (INTER_LINEAR when
+    enlarging), a different filter: flows of a video whose frames are not already `size` differ from the reference's by
+    what the filter changes."""
+    import cv2
+    h, w = size
+    out = []
+    for d in frames:
+        im = np.asarray(d['img_orig'] if 'img_orig' in d else d['img'], np.float32) * 255
+        if im.shape[:2] != (h, w):
+            shrink = im.shape[0] >= h and im.shape[1] >= w
+            im = cv2.resize(im, (w, h), interpolation=cv2.INTER_AREA if shrink else cv2.INTER_LINEAR)
+        out.append(torch.from_numpy(np.ascontiguousarray(im.transpose(2, 0, 1))))
+    return torch.stack(out)
 
 
 class PairBuilder(torch.utils.data.Dataset):
-    def __init__(self, frames_dir, flows_dir, gaps, unit=1.0, device=None, name=None):
+    def __init__(self, frames_dir, flows_dir, gaps, unit=1.0, device=None, name=None, raft=None, raft_iters=20, images=None,
+                 raft_chunk=16):
         """frames_dir: frames_midas/<track>; flows_dir: flow_pairs/<track>; gaps: iterable of frame gaps; unit: 2.0 for a
-        subsampled video (davis_sequence.py:93-96); device: where raw flows are processed (default cuda if available)."""
+        subsampled video (davis_sequence.py:93-96); device: where raw flows are processed (default cuda if available).
+        With flows_dir None the flows are estimated here: raft is a dvd_b200.raft.RaftNet on the device, images the frames at
+        RAFT's resolution ([n,3,h,w] in 0..255, one per frame file in order; default raft_images() of the frame files), and
+        raft_chunk the number of pairs per launch."""
+        if flows_dir is None and raft is None:
+            raise ValueError('PairBuilder needs optical flows: a directory of flowpair_*.npz or a RaftNet to estimate them')
+        if flows_dir is not None and raft is not None:
+            raise ValueError('give either a flow directory or a RaftNet, not both')
         files = sorted(glob.glob(os.path.join(frames_dir, 'frame_*.npz')))
         if not files:
             raise FileNotFoundError('no frame_*.npz under %s' % frames_dir)
@@ -113,7 +146,13 @@ class PairBuilder(torch.utils.data.Dataset):
         self.flows = [None] * len(self.pairs)
         self.raw_pairs = 0
         raw = {}
-        for i, (a, b) in enumerate(self.pairs):
+        if raft is not None:
+            if images is None:
+                images = raft_images([frames[f] for f in used])
+            elif len(images) == len(files):
+                images = images[used]
+            self._estimate_flows(raft, images, used, int(raft_iters), int(raft_chunk))
+        for i, (a, b) in enumerate(self.pairs if raft is None else ()):
             d = read_npz(os.path.join(flows_dir, FLOW_FMT % (a, b)))
             f12, f21 = np.asarray(d['flow_1_2'], np.float32), np.asarray(d['flow_2_1'], np.float32)
             if f12.shape != f21.shape or f12.ndim != 3 or f12.shape[-1] != 2:
@@ -141,6 +180,25 @@ class PairBuilder(torch.utils.data.Dataset):
             for j, (i, _, _) in enumerate(items):
                 self.flows[i] = (f12[j].clone(), f21[j].clone(), m1[j].clone(), m2[j].clone())
             self.raw_pairs += len(items)
+
+    def _estimate_flows(self, raft, images, used, iters, chunk):
+        """RAFT on the device: every frame encoded once, then both directions of all pairs of a gap in chunks, handed to the
+        resize and mask kernels without leaving the device; only the finished flows and masks are copied to the host."""
+        if len(images) != len(used):
+            raise ValueError('%d RAFT images for %d frames' % (len(images), len(used)))
+        dev = next(raft.parameters()).device
+        images = torch.as_tensor(images, dtype=torch.float32)
+        feats = [raft.encode(images[i:i + chunk].to(dev)) for i in range(0, len(images), chunk)]
+        feats = type(feats[0])(torch.cat([f.fmap for f in feats]), torch.cat([f.cnet for f in feats]))
+        slot = {f: k for k, f in enumerate(used)}
+        for i0 in range(0, len(self.pairs), chunk):
+            ids = list(range(i0, min(i0 + chunk, len(self.pairs))))
+            fa, fb = feats.index([slot[self.pairs[i][0]] for i in ids]), feats.index([slot[self.pairs[i][1]] for i in ids])
+            out = finish_flows(raft.flow(fa, fb, iters), raft.flow(fb, fa, iters), self.H, self.W)
+            f12, f21, m1, m2 = (t.cpu() for t in out)
+            for j, i in enumerate(ids):
+                self.flows[i] = (f12[j].clone(), f21[j].clone(), m1[j].clone(), m2[j].clone())
+        self.raw_pairs = len(self.pairs)
 
     def __len__(self):
         return len(self.pairs)

@@ -345,6 +345,62 @@ int dvd_disp_vali_partials_size(int N, int H, int W);
 int dvd_disp_vali(const float* depth, const float* depth_gt, float* frame_sse, float* terms, float* partials, int N, int H, int W,
                   void* stream);
 
+/* ---- RAFT optical flow, forward only (csrc/raft_ops.cu): third_party/RAFT/core as scripts/preprocess/davis/generate_flows.py runs it
+ * (large model, all-pairs correlation, 4 levels, radius 4, hidden = context = 128, no warm start, test_mode). These are the CUDA-core
+ * stages; the convolutions between them are dvd_conv2d_nhwc launches (dvd_b200/raft.py holds the schedule). All tensors NHWC fp32,
+ * 16-byte aligned unless noted; coords1 [B,h,w,2] = (x, y) on the 1/8 grid, 8-byte aligned. Shapes, alignment and byte sizes are
+ * checked before any launch (-2 with a message). No kernel uses atomics: equal inputs give bitwise equal outputs.
+ * `round_out` = 1 stores TF32-rounded values (the tensor feeds a tensor-core convolution).                                      */
+/* y [N,H/2,W/2,64] = conv7x7/2 pad 3 (2 (x / 255) - 1) + bias: extractor.py BasicEncoder.conv1 with raft.py:88-89 folded in.
+ * x_nchw [N,3,H,W] holds 0..255; weight [64,3,7,7] and bias [64] contiguous. (The BatchNorm encoder's stem is dvd_stem_fwd.)     */
+int dvd_raft_stem_fwd(const float* x_nchw, const float* weight, const float* bias, float* y, size_t y_bytes, int N, int H, int W,
+                      void* stream);
+/* nn.InstanceNorm2d (no affine, biased variance): stats [N,C,2] = (mean, 1 / sqrt(var + eps)) of x [N,P,C] per image and channel.
+ * Two kernels with a fixed reduction order and fp64 sums; scratch: dvd_raft_instnorm_scratch_bytes(N, C) bytes.                  */
+long dvd_raft_instnorm_scratch_bytes(int N, int C);
+int dvd_raft_instnorm_stats(const float* x, float* stats, void* scratch, size_t scratch_bytes, int N, long P, int C, float eps,
+                            void* stream);
+/* y = relu_outer?( relu_inner?( (x - mean) * rstd ) + res ): the norm + ReLU + residual add + ReLU of extractor.py ResidualBlock.
+ * stats NULL: no normalisation (the BatchNorm encoder's residual add); res NULL: no add. y may alias x.                            */
+int dvd_raft_norm_act(const float* x, const float* stats, const float* res, float* y, int N, long P, int C, int relu_inner,
+                      int relu_outer, int round_out, void* stream);
+/* corr.py CorrBlock.__init__: level 0 [B, h w, h, w] = <fmap1[b,p,:], fmap2[b,q,:]> / sqrt(C) in plain fp32 FMA (the lookup
+ * differentiates this volume, so no TF32 product), then three 2 x 2 average poolings over q. The levels are stored one after another,
+ * dvd_raft_pyramid_floats(B, h, w) floats in all (-1 unless every level is at least 2 x 2, i.e. h, w >= 16: the reference's
+ * lookup divides by (w - 1) and (h - 1) of every level). fmap [B,h,w,C], 16 | C.                                                */
+long dvd_raft_pyramid_floats(int B, int h, int w);
+int dvd_raft_corr_pyramid(const float* fmap1, const float* fmap2, float* pyramid, size_t pyramid_bytes, int B, int h, int w, int C,
+                          void* stream);
+/* corr.py CorrBlock.__call__ for all four levels in one launch: out [B,h,w,352], channel l * 81 + i * 9 + j = bilinear sample
+ * (zeros outside) of level l at (x / 2^l + i - 4, y / 2^l + j - 4) - the window's slow index moves along x, as the reference's
+ * meshgrid(dy, dx) added to (x, y) does; channels 324..351 are zero (the 1x1 convolution behind it wants 32 | Cin).              */
+int dvd_raft_lookup(const float* pyramid, size_t pyramid_bytes, const float* coords1, float* out, size_t out_bytes, int B, int h,
+                    int w, int round_out, void* stream);
+/* update.py BasicMotionEncoder.convf1 + ReLU: y [B,h,w,128] = relu(conv7x7 pad 3 (coords1 - grid)); weight [128,2,7,7], bias [128] */
+int dvd_raft_convf1(const float* coords1, const float* weight, const float* bias, float* y, int B, int h, int w, int round_out,
+                    void* stream);
+/* The GRU's operands are X = [h | inp | motion] and XR = [r h | inp | motion], [npx,384] each, written in place (no cat):
+ * context_split: cnet [npx,256] (context encoder output) -> net = tanh(first half) [npx,128] (kept un-rounded: the hidden state),
+ *   X[:, 0:128] = round(net), X / XR[:, 128:256] = round(relu(second half))                            (raft.py:109-113)
+ * motion_pack:   X / XR[:, 256:384] = [mconv[:, 0:126] | round(coords1 - grid)], mconv [npx,128] the 126-output convolution of
+ *   BasicMotionEncoder padded to 128 (already ReLU'd and rounded)                                      (update.py:95-97)
+ * gru_rh:        XR[:, 0:128] = round(sigmoid(zr[:, 128:256]) * net), zr [npx,256] = pre-activations of convz | convr
+ * gru_update:    net = (1 - z) net + z tanh(q), z = sigmoid(zr[:, 0:128]), q [npx,128] the pre-activation of convq;
+ *   X[:, 0:128] = round(net) and, when not NULL, net_r [npx,128] = round(net)                          (update.py:49-61)         */
+int dvd_raft_context_split(const float* cnet, float* net, float* X, float* XR, long npx, void* stream);
+int dvd_raft_motion_pack(const float* mconv, const float* coords1, float* X, float* XR, int B, int h, int w, void* stream);
+int dvd_raft_gru_rh(const float* zr, const float* net, float* XR, long npx, void* stream);
+int dvd_raft_gru_update(const float* zr, const float* q, float* net, float* X, float* net_r, long npx, void* stream);
+/* update.py FlowHead.conv2 + raft.py:131: delta = conv3x3 pad 1 (x) + bias, x [B,h,w,256], weight [2,256,3,3]; coords1 += delta in
+ * place; delta [B,h,w,2] is also stored unless NULL.                                                                          */
+int dvd_raft_flow_head(const float* x, const float* weight, const float* bias, float* coords1, float* delta, int B, int h, int w,
+                       void* stream);
+/* raft.py upsample_flow: flow [B,8h,8w,2] = sum_k softmax_k(mask_scale * mask[k*64 + i*8 + j]) * 8 (coords1 - grid)[neighbour k]
+ * (3 x 3, zeros outside). The 576 mask channels come as three [B,h,w,192] tensors (the convolution kernel's widths do not include
+ * 576); mask_scale = 0.25 for the raw output of update_block.mask (update.py:136).                                            */
+int dvd_raft_upsample(const float* mask0, const float* mask1, const float* mask2, const float* coords1, float* flow,
+                      size_t flow_bytes, int B, int h, int w, float mask_scale, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
