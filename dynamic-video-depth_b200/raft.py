@@ -64,6 +64,9 @@ class _Encoder(nn.Module):
         return list(self.layer1) + list(self.layer2) + list(self.layer3)
 
 
+BLOCK_NAMES = ('layer1.0', 'layer1.1', 'layer2.0', 'layer2.1', 'layer3.0', 'layer3.1')     # _Encoder.blocks(), the reference's names
+
+
 class _MotionEncoder(nn.Module):
     def __init__(self):
         super().__init__()
@@ -206,6 +209,12 @@ def upsample(masks, coords1, mask_scale=0.25):
     return flow
 
 
+def _keep(trace, name, t):
+    """trace[name] = a copy of t as it is now: X, XR, net and coords1 are overwritten in place later in the same iteration"""
+    if trace is not None:
+        trace[name] = t.clone()
+
+
 def coords_grid(B, h, w, device):
     ys, xs = torch.meshgrid(torch.arange(h, dtype=torch.float32, device=device), torch.arange(w, dtype=torch.float32, device=device),
                             indexing='ij')
@@ -311,9 +320,10 @@ class RaftNet(nn.Module):
         check_size(images.shape[2], images.shape[3])
         return images.contiguous()
 
-    def feature_stem(self, images):
+    def feature_stem(self, images, trace=None):
         """relu(InstanceNorm(conv1(2 (x / 255) - 1))) of the feature encoder, [N,H/2,W/2,64]"""
         s = raft_stem(images, self.fnet.conv1.weight.detach().contiguous(), self.fnet.conv1.bias.detach())
+        _keep(trace, 'fnet.stem', s)
         return norm_act(s, instnorm_stats(s), relu_inner=True)
 
     def context_stem(self, images):
@@ -323,72 +333,114 @@ class RaftNet(nn.Module):
         return y.permute(0, 2, 3, 1)          # channels-last memory: a contiguous [N,H/2,W/2,64] view
 
     @torch.no_grad()
-    def encode(self, images):
-        """images [N,3,H,W] fp32 in 0..255 on the device -> FrameFeatures of the N frames"""
+    def encode(self, images, trace=None):
+        """images [N,3,H,W] fp32 in 0..255 on the device -> FrameFeatures of the N frames. trace: None, or a dict that receives
+        a copy of every intermediate tensor under the names of oracle/raft_tf32.py (NHWC)"""
         images = self._check_images(images)
         P = self.plan()
         prev = conv_ops.set_workspace_lane(-1)
         try:
-            x = self.feature_stem(images)
-            for c1, c2, ds in P.f_blocks:
+            x = self.feature_stem(images, trace)
+            _keep(trace, 'fnet.stem.out', x)
+            for name, (c1, c2, ds) in zip(BLOCK_NAMES, P.f_blocks):
+                p = 'fnet.' + name + '.'
                 a = c1(x)
                 y = norm_act(a, instnorm_stats(a), relu_inner=True)
                 b = c2(y)
+                _keep(trace, p + 'a', a)
+                _keep(trace, p + 'y', y)
+                _keep(trace, p + 'b', b)
                 if ds is None:
                     x = norm_act(b, instnorm_stats(b), res=x, relu_inner=True, relu_outer=True)
                 else:
                     yb = norm_act(b, instnorm_stats(b), relu_inner=True, round_out=False)
                     d = ds(x)
                     x = norm_act(d, instnorm_stats(d), res=yb, relu_outer=True)
+                    _keep(trace, p + 'yb', yb)
+                    _keep(trace, p + 'd', d)
+                _keep(trace, p + 'out', x)
             fmap = P.f_out(x)
+            _keep(trace, 'fmap', fmap)
             x = self.context_stem(images)
-            for c1, c2, ds in P.c_blocks:
-                b = c2(c1(x))
+            _keep(trace, 'cnet.stem.out', x)
+            for name, (c1, c2, ds) in zip(BLOCK_NAMES, P.c_blocks):
+                p = 'cnet.' + name + '.'
+                y = c1(x)
+                b = c2(y)
                 # relu(x + relu(bn2(conv2))): the shortcut is added after the branch's own ReLU, so it is not the convolution's residual
                 x = norm_act(b, res=x, relu_outer=True) if ds is None else ds(x, res=b)
-            return FrameFeatures(fmap, P.c_out(x))
+                _keep(trace, p + 'y', y)
+                _keep(trace, p + 'b', b)
+                _keep(trace, p + 'out', x)
+            cnet = P.c_out(x)
+            _keep(trace, 'cnet', cnet)
+            return FrameFeatures(fmap, cnet)
         finally:
             conv_ops.set_workspace_lane(prev)
 
     # -- update iterations ----------------------------------------------------------------------------
-    def update_step(self, P, pyr, coords1, net, X, XR, net_r, want_delta=False):
-        """one iteration in place: coords1, net, X, XR, net_r are overwritten; returns (lookup output, delta_flow or None)"""
+    def update_step(self, P, pyr, coords1, net, X, XR, net_r, want_delta=False, trace=None):
+        """one iteration in place: coords1, net, X, XR, net_r are overwritten; returns (lookup output, delta_flow or None).
+        trace: None, or a dict that receives a copy of every tensor of the iteration (names of oracle/raft_tf32.py, NHWC; the
+        operand buffers as 'X.<stage>' / 'XR.<stage>' after each kernel that writes them)"""
         B, h, w, _ = coords1.shape
         npx = B * h * w
         e = self.update_block.encoder
         corr = lookup(pyr, coords1)
-        cor = P.convc2(P.convc1(corr))
+        c1 = P.convc1(corr)
+        cor = P.convc2(c1)
         flo = torch.empty(B, h, w, 128, dtype=torch.float32, device=coords1.device)
         _raft('dvd_raft_convf1', _ptr(coords1), _ptr(e.convf1.weight.detach().contiguous()), _ptr(e.convf1.bias.detach()), _ptr(flo), B, h, w, 1)
-        m = P.conv_cor(cor, res=P.conv_flo(P.convf2(flo)))
+        f2 = P.convf2(flo)
+        m = P.conv_cor(cor, res=P.conv_flo(f2))
         _raft('dvd_raft_motion_pack', _ptr(m), _ptr(coords1), _ptr(X), _ptr(XR), B, h, w)
+        if trace is not None:
+            for name, t in (('corr', corr), ('convc1', c1), ('convc2', cor), ('convf1', flo), ('convf2', f2), ('motion', m),
+                            ('X.pack', X), ('XR.pack', XR)):
+                _keep(trace, name, t)
         for i, (zr_conv, q_conv) in enumerate(P.gru):
             zr = zr_conv(X)
             _raft('dvd_raft_gru_rh', _ptr(zr), _ptr(net), _ptr(XR), npx)
+            _keep(trace, 'XR.rh.%d' % i, XR)
             q = q_conv(XR)
             _raft('dvd_raft_gru_update', _ptr(zr), _ptr(q), _ptr(net), _ptr(X), _ptr(net_r if i == 1 else None), npx)
+            if trace is not None:
+                for name, t in (('zr', zr), ('q', q), ('net', net), ('X.gru', X)):
+                    _keep(trace, '%s.%d' % (name, i), t)
         fh = P.fh1(net_r)
         fhc = self.update_block.flow_head.conv2
-        delta = torch.empty(B, h, w, 2, dtype=torch.float32, device=coords1.device) if want_delta else None
+        delta = torch.empty(B, h, w, 2, dtype=torch.float32, device=coords1.device) if want_delta or trace is not None else None
         _raft('dvd_raft_flow_head', _ptr(fh), _ptr(fhc.weight.detach().contiguous()), _ptr(fhc.bias.detach()), _ptr(coords1), _ptr(delta), B, h, w)
+        if trace is not None:
+            for name, t in (('net_r', net_r), ('fh', fh), ('delta', delta), ('coords1', coords1)):
+                _keep(trace, name, t)
         return corr, delta
 
-    def init_state(self, cnet):
+    def init_state(self, cnet, trace=None):
         """cnet [B,h,w,256] -> (net [B,h,w,128], X, XR [B,h,w,384], net_r [B,h,w,128]) with the tanh / relu halves in place"""
         B, h, w, _ = cnet.shape
         dev = cnet.device
         net, net_r = (torch.empty(B, h, w, 128, dtype=torch.float32, device=dev) for _ in range(2))
         X, XR = (torch.empty(B, h, w, 384, dtype=torch.float32, device=dev) for _ in range(2))
         _raft('dvd_raft_context_split', _ptr(cnet), _ptr(net), _ptr(X), _ptr(XR), B * h * w)
+        if trace is not None:
+            for name, t in (('net', net), ('X', X), ('XR', XR)):
+                _keep(trace, name, t)
         return net, X, XR, net_r
 
-    def mask_parts(self, P, net_r):
+    def mask_parts(self, P, net_r, trace=None):
         mk = P.mask0(net_r)
-        return [c(mk) for c in P.mask2]
+        parts = [c(mk) for c in P.mask2]
+        if trace is not None:
+            _keep(trace, 'mask0', mk)
+            trace['mask'] = [t.clone() for t in parts]
+        return parts
 
     @torch.no_grad()
-    def flow(self, feat_a, feat_b, iters=20, return_low=False):
-        """flow from the frames of feat_a to those of feat_b, pair by pair: [B,H,W,2] fp32 (x, y), the layout of the flow-pair kernels"""
+    def flow(self, feat_a, feat_b, iters=20, return_low=False, trace=None):
+        """flow from the frames of feat_a to those of feat_b, pair by pair: [B,H,W,2] fp32 (x, y), the layout of the flow-pair kernels.
+        trace: None, or a dict that receives 'pyramid' (the flat buffer), the initial state ('net', 'X', 'XR'), one dict per
+        iteration under 'iters' (see update_step), the mask head ('mask0', 'mask': the three parts) and 'flow_up'"""
         iters = int(iters)
         if iters < 1:
             raise ValueError('iters must be at least 1')
@@ -400,11 +452,17 @@ class RaftNet(nn.Module):
             fa, fb, cn = feat_a.fmap.contiguous(), feat_b.fmap.contiguous(), feat_a.cnet.contiguous()
             B, h, w, _ = fa.shape
             pyr = corr_pyramid(fa, fb)
-            net, X, XR, net_r = self.init_state(cn)
+            _keep(trace, 'pyramid', pyr)
+            net, X, XR, net_r = self.init_state(cn, trace)
             coords1 = coords_grid(B, h, w, fa.device)
             for _ in range(iters):
-                self.update_step(P, pyr, coords1, net, X, XR, net_r)
-            up = upsample(self.mask_parts(P, net_r), coords1)
+                it = None
+                if trace is not None:
+                    it = {}
+                    trace.setdefault('iters', []).append(it)
+                self.update_step(P, pyr, coords1, net, X, XR, net_r, trace=it)
+            up = upsample(self.mask_parts(P, net_r, trace), coords1)
+            _keep(trace, 'flow_up', up)
             return (up, coords1 - coords_grid(B, h, w, fa.device)) if return_low else up
         finally:
             conv_ops.set_workspace_lane(prev)
