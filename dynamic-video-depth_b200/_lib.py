@@ -123,12 +123,21 @@ SIGNATURES = {
     'dvd_raft_gru_update': [_P, _P, _P, _P, _P, ctypes.c_long, _P],
     'dvd_raft_flow_head': [_P, _P, _P, _P, _P, _I, _I, _I, _P],
     'dvd_raft_upsample': [_P, _P, _P, _P, _P, ctypes.c_size_t, _I, _I, _I, _F, _P],
+    'dvd_resize_bicubic_ac': [_P, ctypes.c_size_t, _P, ctypes.c_size_t, _I, _I, _I, _I, _I, _P],
+    'dvd_spline_prefilter': [_P, ctypes.c_size_t, _P, ctypes.c_size_t, _I, _I, _I, _P],
+    'dvd_spline_sample': [_P, ctypes.c_size_t, _I, _I, _I, _P, _P, ctypes.c_long, _P],
+    'dvd_calib_ratios': [_P, _P, ctypes.c_size_t, _P, _P, ctypes.c_long, ctypes.c_double, ctypes.c_double, ctypes.c_double,
+                         ctypes.c_double, _P, ctypes.c_size_t, _I, _I, _I, _P],
+    'dvd_sorted_median': [_P, ctypes.c_size_t, _I, ctypes.c_long, _P, _P, _P],
+    'dvd_aa_resize_scratch_bytes': [_I, _I, _I, _I],
+    'dvd_aa_resize': [_P, ctypes.c_size_t, _P, ctypes.c_size_t, _P, ctypes.c_size_t, _P, _I, _P, _I, _I, _I, _I, _I, _I, _I, _P],
 }
 DVD_MASKS_FLOWPAIR_U8 = 0
 DVD_MASKS_PAIRFILE_F32 = 1
 _RESTYPES = {'dvd_last_error': ctypes.c_char_p, 'dvd_struct_size': ctypes.c_long, 'dvd_conv2d_workspace_bytes': ctypes.c_size_t, 'dvd_conv2d_pack_blocks': ctypes.c_long, 'dvd_mlp_packed_weights_bytes': ctypes.c_size_t,
              'dvd_mlp_save_bytes_per_eval': ctypes.c_size_t, 'dvd_mlp_dy_bytes': ctypes.c_size_t,
-             'dvd_raft_instnorm_scratch_bytes': ctypes.c_long, 'dvd_raft_pyramid_floats': ctypes.c_long}
+             'dvd_raft_instnorm_scratch_bytes': ctypes.c_long, 'dvd_raft_pyramid_floats': ctypes.c_long,
+             'dvd_aa_resize_scratch_bytes': ctypes.c_long}
 
 _lib = None
 

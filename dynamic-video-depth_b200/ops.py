@@ -656,3 +656,141 @@ def disp_vali(depth, depth_gt, want_terms=False, out=None):
     _lib.check(lib.dvd_disp_vali(_ptr(depth), _ptr(depth_gt), _ptr(out), _ptr(terms), _ptr(partials), N, H, W, _stream()),
                'dvd_disp_vali')
     return (out, terms) if want_terms else out
+
+
+# ---- frame preparation (csrc/frame_prep.cu) ---------------------------------------------------------------------------------
+def _chk_dtype(t, name, dtype, dim):
+    if not isinstance(t, torch.Tensor) or not t.is_cuda:
+        raise ValueError('%s must be a CUDA tensor (dvd_b200 has no CPU path)' % name)
+    if t.dtype != dtype or not t.is_contiguous() or t.dim() != dim:
+        raise ValueError('%s must be a contiguous %d-d %s tensor, got %s %s' % (name, dim, dtype, t.dtype, tuple(t.shape)))
+    return t
+
+
+def resize_bicubic_ac(x, H, W):
+    """F.interpolate(x, (H, W), mode='bicubic', align_corners=True) of a [N,C,h,w] fp32 tensor, any sizes."""
+    _chk(x, 'x')
+    if x.dim() != 4:
+        raise ValueError('x must be [N,C,h,w], got %s' % (tuple(x.shape),))
+    H, W = int(H), int(W)
+    if H < 1 or W < 1:
+        raise ValueError('output size must be positive, got %dx%d' % (H, W))
+    N, C, h, w = x.shape
+    out = torch.empty(N, C, H, W, dtype=torch.float32, device=x.device)
+    LAUNCHES['n'] += 1
+    _lib.check(_lib.load().dvd_resize_bicubic_ac(_ptr(x), x.numel() * 4, _ptr(out), out.numel() * 4, N * C, h, w, H, W, _stream()),
+               'dvd_resize_bicubic_ac')
+    return out
+
+
+def spline_prefilter(maps, out=None):
+    """scipy.ndimage.spline_filter(m, 3, output=float64, mode='constant') of each [H,W] map of [N,H,W] fp32 -> fp64 [N,H,W]."""
+    _chk(maps, 'maps')
+    if maps.dim() != 3:
+        raise ValueError('maps must be [N,H,W], got %s' % (tuple(maps.shape),))
+    if out is None:
+        out = torch.empty(maps.shape, dtype=torch.float64, device=maps.device)
+    elif _chk_dtype(out, 'out', torch.float64, 3).shape != maps.shape:
+        raise ValueError('out %s must match maps %s' % (tuple(out.shape), tuple(maps.shape)))
+    N, H, W = maps.shape
+    LAUNCHES['n'] += 2
+    _lib.check(_lib.load().dvd_spline_prefilter(_ptr(maps), maps.numel() * 4, _ptr(out), out.numel() * 8, N, H, W, _stream()),
+               'dvd_spline_prefilter')
+    return out
+
+
+def spline_sample(coef, vu):
+    """map_coordinates(map[n], [v, u], order=3, mode='constant') from spline_prefilter's coef [N,H,W] at vu [N,P,2] fp64 (v, u)
+    -> [N,P] fp32; coordinates outside the map, NaN or inf give 0."""
+    _chk_dtype(coef, 'coef', torch.float64, 3)
+    _chk_dtype(vu, 'vu', torch.float64, 3)
+    N, H, W = coef.shape
+    if vu.shape[0] != N or vu.shape[2] != 2 or vu.shape[1] < 1 or vu.device != coef.device:
+        raise ValueError('vu must be [%d,P,2] on %s, got %s' % (N, coef.device, tuple(vu.shape)))
+    P = vu.shape[1]
+    out = torch.empty(N, P, dtype=torch.float32, device=coef.device)
+    LAUNCHES['n'] += 1
+    _lib.check(_lib.load().dvd_spline_sample(_ptr(coef), coef.numel() * 8, N, H, W, _ptr(vu), _ptr(out), P, _stream()),
+               'dvd_spline_sample')
+    return out
+
+
+def calib_ratios(depth_coef, mask_coef, w2c, points, fx, fy, cx, cy, out=None):
+    """The reference's per-frame point selection and nn / depth ratios (generate_frame_midas.py:81-101): depth_coef, mask_coef
+    [N,H,W] fp64 (spline_prefilter of the full-resolution depth and mask), w2c [N,4,4] fp64, points [V,3] fp64 -> ratio [N,V]
+    fp64, NaN for a rejected point. `out` may be a caller-owned [N,V] fp64 buffer (e.g. rows of a longer one)."""
+    _chk_dtype(depth_coef, 'depth_coef', torch.float64, 3)
+    _chk_dtype(mask_coef, 'mask_coef', torch.float64, 3)
+    _chk_dtype(w2c, 'w2c', torch.float64, 3)
+    _chk_dtype(points, 'points', torch.float64, 2)
+    N, H, W = depth_coef.shape
+    dev = depth_coef.device
+    if mask_coef.shape != depth_coef.shape or tuple(w2c.shape) != (N, 4, 4) or points.shape[1] != 3 or points.shape[0] < 1:
+        raise ValueError('bad shapes: depth_coef %s, mask_coef %s, w2c %s, points %s' % (
+            tuple(depth_coef.shape), tuple(mask_coef.shape), tuple(w2c.shape), tuple(points.shape)))
+    if any(t.device != dev for t in (mask_coef, w2c, points)):
+        raise ValueError('all tensors must be on %s' % dev)
+    V = points.shape[0]
+    if out is None:
+        out = torch.empty(N, V, dtype=torch.float64, device=dev)
+    elif tuple(_chk_dtype(out, 'out', torch.float64, 2).shape) != (N, V):
+        raise ValueError('out must be [%d,%d], got %s' % (N, V, tuple(out.shape)))
+    LAUNCHES['n'] += 1
+    _lib.check(_lib.load().dvd_calib_ratios(_ptr(depth_coef), _ptr(mask_coef), depth_coef.numel() * 8, _ptr(w2c), _ptr(points), V,
+                                            float(fx), float(fy), float(cx), float(cy), _ptr(out), out.numel() * 8, N, H, W,
+                                            _stream()), 'dvd_calib_ratios')
+    return out
+
+
+def row_medians(ratio):
+    """np.median of the non-NaN entries of each row of [N,V] fp64 -> (median [N] fp64, count [N] int32). The rows are sorted on
+    the device first (NaN last)."""
+    _chk_dtype(ratio, 'ratio', torch.float64, 2)
+    N, V = ratio.shape
+    srt = torch.sort(ratio, dim=1)[0].contiguous()
+    med = torch.empty(N, dtype=torch.float64, device=ratio.device)
+    cnt = torch.empty(N, dtype=torch.int32, device=ratio.device)
+    LAUNCHES['n'] += 1
+    _lib.check(_lib.load().dvd_sorted_median(_ptr(srt), srt.numel() * 8, N, V, _ptr(med), _ptr(cnt), _stream()), 'dvd_sorted_median')
+    return med, cnt
+
+
+def gaussian_weights(n_in, n_out):
+    """skimage's anti-aliasing kernel along an axis shrunk from n_in to n_out: sigma = max(0, (n_in / n_out - 1) / 2), then
+    scipy.ndimage's gaussian_filter1d weights (truncate 4: radius int(4 sigma + 0.5), exp(-x² / (2 sigma²)) normalised by its sum).
+    An axis with sigma <= 1e-15 is not filtered by scipy: the single weight 1 leaves it unchanged. Returns (radius, fp64 weights)."""
+    import numpy as np
+    sigma = max(0.0, (float(np.divide(n_in, n_out)) - 1.0) / 2.0)
+    if sigma <= 1e-15:
+        return 0, np.ones(1)
+    radius = int(4.0 * sigma + 0.5)
+    x = np.arange(-radius, radius + 1)
+    phi = np.exp(-0.5 / (sigma * sigma) * x ** 2)
+    return radius, phi / phi.sum()
+
+
+def aa_resize(src, OH, OW, weights=None):
+    """skimage.transform.resize(img, (OH, OW), preserve_range=True) (skimage >= 0.19: Gaussian anti-aliasing when shrinking, order 1,
+    mode 'reflect', clip) of each frame of a [N,H,W,C] fp32 tensor -> [N,OH,OW,C] fp32. `weights` = the two fp64 device weight
+    tensors of gaussian_weights (built here when None)."""
+    _chk(src, 'src')
+    if src.dim() != 4:
+        raise ValueError('src must be [N,H,W,C], got %s' % (tuple(src.shape),))
+    OH, OW = int(OH), int(OW)
+    if OH < 1 or OW < 1:
+        raise ValueError('output size must be positive, got %dx%d' % (OH, OW))
+    N, H, W, C = src.shape
+    if weights is None:
+        weights = [torch.from_numpy(gaussian_weights(n, o)[1]).to(src.device) for n, o in ((H, OH), (W, OW))]
+    wy, wx = weights
+    for name, t in (('wy', wy), ('wx', wx)):
+        if _chk_dtype(t, name, torch.float64, 1).numel() % 2 == 0:
+            raise ValueError('%s must have an odd length 2 r + 1' % name)
+    lib = _lib.load()
+    nb = lib.dvd_aa_resize_scratch_bytes(N, H, W, C)
+    scratch = torch.empty(nb // 4, dtype=torch.float32, device=src.device)
+    out = torch.empty(N, OH, OW, C, dtype=torch.float32, device=src.device)
+    LAUNCHES['n'] += 4
+    _lib.check(lib.dvd_aa_resize(_ptr(src), src.numel() * 4, _ptr(out), out.numel() * 4, _ptr(scratch), nb, _ptr(wy),
+                                 wy.numel() // 2, _ptr(wx), wx.numel() // 2, N, H, W, C, OH, OW, _stream()), 'dvd_aa_resize')
+    return out

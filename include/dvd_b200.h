@@ -345,6 +345,37 @@ int dvd_disp_vali_partials_size(int N, int H, int W);
 int dvd_disp_vali(const float* depth, const float* depth_gt, float* frame_sse, float* terms, float* partials, int N, int H, int W,
                   void* stream);
 
+/* ---- frame preparation (csrc/frame_prep.cu): scripts/preprocess/davis/generate_frame_midas.py ---------------------------------
+ * Buffers are caller-allocated; byte sizes, shapes and alignment are checked before any launch (-2 with a message); nothing
+ * synchronises. The scipy stages accumulate in fp64 and round to fp32 where scipy stores fp32.                                */
+/* F.interpolate(x, (H, W), mode='bicubic', align_corners=True) of NC planes: src [NC,h,w] -> dst [NC,H,W] fp32, any sizes (ATen's
+ * upsample_bicubic2d: fp32 scale (in - 1) / (out - 1), A = -0.75, taps clamped to the border).                                 */
+int dvd_resize_bicubic_ac(const float* src, size_t src_bytes, float* dst, size_t dst_bytes, int NC, int h, int w, int H, int W,
+                          void* stream);
+/* scipy.ndimage.spline_filter(maps[n], 3, output=float64, mode='constant') for n < N: maps [N,H,W] fp32 -> coef [N,H,W] fp64,
+ * recursive prefilter along axis 0, then axis 1.                                                                              */
+int dvd_spline_prefilter(const float* maps, size_t maps_bytes, double* coef, size_t coef_bytes, int N, int H, int W, void* stream);
+/* map_coordinates(maps[n], [v, u], order=3, mode='constant') from coef [N,H,W]: vu [N,P,2] fp64 (v, u) pairs, 16-byte aligned ->
+ * out [N,P] fp32. A coordinate outside [0, H-1] x [0, W-1], NaN or inf gives 0.                                               */
+int dvd_spline_sample(const double* coef, size_t coef_bytes, int N, int H, int W, const double* vu, float* out, long P, void* stream);
+/* Scale calibration, one thread per (frame n, point p): out = w2c[n] [X;1] (w2c [N,4,4] fp64 row-major, points [V,3] fp64),
+ * (u, v) = (fx out.x + cx out.z, fy out.y + cy out.z) / out.z, depth = out.z. The point is kept when 0 <= u < W and 0 <= v < H,
+ * then when map_coordinates(mask, [v, u]) < 0.1f, then when depth > 1e-3; ratio [N,V] = (double)map_coordinates(depth, [v, u])
+ * / depth for a kept point, NaN otherwise. depth_coef and mask_coef are dvd_spline_prefilter outputs of the same [N,H,W] shape. */
+int dvd_calib_ratios(const double* depth_coef, const double* mask_coef, size_t coef_bytes, const double* w2c, const double* points,
+                     long V, double fx, double fy, double cx, double cy, double* ratio, size_t ratio_bytes, int N, int H, int W,
+                     void* stream);
+/* np.median of the non-NaN entries of each row of sorted [N,V] (rows ascending, NaN last): median [N] fp64, count [N] int32
+ * (the number of non-NaN entries; the median is NaN where it is 0).                                                           */
+int dvd_sorted_median(const double* sorted, size_t sorted_bytes, int N, long V, double* median, int* count, void* stream);
+/* skimage.transform.resize(src[n], (OH, OW), preserve_range=True) of fp32 [N,H,W,C] as skimage >= 0.19 computes it:
+ * gaussian_filter along axis 0 with the weights wy [2 ry + 1], then axis 1 with wx [2 rx + 1] (fp64 device arrays; mode 'mirror',
+ * each pass fp64 and stored fp32), zoom(order=1, mode='mirror', grid_mode=True) in fp64 rounded to fp32, then a clip to the
+ * frame's input min / max. scratch: dvd_aa_resize_scratch_bytes(N, H, W, C) bytes (-1 for a bad shape), 4-byte aligned.       */
+long dvd_aa_resize_scratch_bytes(int N, int H, int W, int C);
+int dvd_aa_resize(const float* src, size_t src_bytes, float* dst, size_t dst_bytes, void* scratch, size_t scratch_bytes,
+                  const double* wy, int ry, const double* wx, int rx, int N, int H, int W, int C, int OH, int OW, void* stream);
+
 /* ---- RAFT optical flow, forward only (csrc/raft_ops.cu): third_party/RAFT/core as scripts/preprocess/davis/generate_flows.py runs it
  * (large model, all-pairs correlation, 4 levels, radius 4, hidden = context = 128, no warm start, test_mode). These are the CUDA-core
  * stages; the convolutions between them are dvd_conv2d_nhwc launches (dvd_b200/raft.py holds the schedule). All tensors NHWC fp32,
