@@ -94,7 +94,6 @@ SIGNATURES = {
     'dvd_conv2d_pack_batch': [_P, _I, ctypes.c_long, _I, _P],
     'dvd_conv2d_wgrad': [ctypes.POINTER(ConvDesc), _P, _P, _P, _P, ctypes.c_long, ctypes.c_long, ctypes.c_long, ctypes.c_long,
                          _I, _I, _P, _P, _P, _P, _P, _P],
-    'dvd_conv2d_cluster_info': [ctypes.POINTER(ctypes.c_int)],
     'dvd_round_tf32': [_P, _P, ctypes.c_long, _P],
     'dvd_relu_bwd_colsum': [_P, _P, _P, _P, _P, _P, _F, _P, ctypes.c_long, _I, _I, _P],
     'dvd_maxpool3x3s2_fwd': [_P, _P, _P, _I, _I, _I, _I, _P],

@@ -93,46 +93,37 @@ def make_desc(N, H, W, Cin, OH, OW, Cout, taps, stride=1, kblock=0, YH=None, YW=
 # ------------------------------------------------------------------------------------------------
 # raw launches
 
-_WORKSPACE = {}     # (device index, lane) -> zero-initialised exchange area of the stream-K schedule (dvd_conv2d_nhwc_ws)
-_WS_LANE = 0
-
-
-def set_workspace_lane(lane):
-    """Convolutions that may run CONCURRENTLY (the lanes of depth_engine.MidasEngine: one stream each) must not share an exchange
-    area; launches of one lane are stream-ordered. lane < 0: no exchange area, i.e. no stream-K schedule - used while SEVERAL
-    lanes are active: a stream-K launch spins in its finishing CTAs until the CTAs that hold the rest of their tiles have run, which
-    is only deadlock-free when no other spinning launch can occupy the SMs those CTAs are waiting for. Returns the previous lane."""
-    global _WS_LANE
-    prev, _WS_LANE = _WS_LANE, int(lane)
-    return prev
+_WORKSPACE = {}     # device index -> zero-initialised exchange area of the stream-K schedule (dvd_conv2d_nhwc_ws)
 
 
 def conv_workspace(device):
-    """The exchange area of the convolution kernel's stream-K schedule for the current lane of this device. All convolutions of a
-    lane are issued on one stream at a time (the current stream, or the capture stream of the step graph); a caller that runs
-    convolutions concurrently on several streams outside the engine's lanes must set DVD_CONV_STREAMK=0. Never allocated during a
-    graph capture (the eager warm-up steps before a capture have the same lanes)."""
-    if _WS_LANE < 0:
-        return None
-    idx = (device.index if device.index is not None else torch.cuda.current_device(), _WS_LANE)
+    """The exchange area of the convolution kernel's stream-K schedule on this device, one for every caller that passes it to
+    conv2d_launch. Never allocated during a graph capture (the eager warm-up steps before a capture allocate it)."""
+    idx = device.index if device.index is not None else torch.cuda.current_device()
     ws = _WORKSPACE.get(idx)
     if ws is None:
         if torch.cuda.is_current_stream_capturing():
             return None
-        ws = torch.zeros(_lib.load().dvd_conv2d_workspace_bytes() // 4, dtype=torch.float32, device=torch.device('cuda', idx[0]))
-        torch.cuda.current_stream(idx[0]).synchronize()
+        ws = torch.zeros(_lib.load().dvd_conv2d_workspace_bytes() // 4, dtype=torch.float32, device=torch.device('cuda', idx))
+        torch.cuda.current_stream(idx).synchronize()
         _WORKSPACE[idx] = ws
     return ws
 
 
-def conv2d_launch(desc, x, w_img, y, bias=None, bn=None, res=None, res2=None, mask=None, flops=0.0, kind='conv'):
+def conv2d_launch(desc, x, w_img, y, bias=None, bn=None, res=None, res2=None, mask=None, flops=0.0, kind='conv', workspace=None):
+    """One tensor-core convolution. workspace=None runs whole tiles only, so a pixel's sum order does not depend on the other
+    pixels of the launch. With conv_workspace(device) the layers whose whole tiles would leave much of the machine idle take the
+    stream-K schedule instead. The caller must guarantee that launches sharing an exchange area are ordered on one stream, and a
+    caller that runs convolutions concurrently on several streams passes none: a stream-K launch spins in its finishing CTAs until
+    the CTAs holding the rest of their tiles have run, which is only deadlock-free when no other spinning launch can occupy the SMs
+    those CTAs wait for."""
     g, b, m, v = bn if bn is not None else (None, None, None, None)
     LAUNCHES['n'] += 1
     ev = _prof(kind, flops, desc)
-    ws = conv_workspace(x.device)
+    ws_bytes = workspace.numel() * 4 if workspace is not None else 0
     _lib.check(_lib.load().dvd_conv2d_nhwc_ws(ctypes.byref(desc), _ptr(x), _ptr(w_img), _ptr(bias), _ptr(g), _ptr(b), _ptr(m), _ptr(v),
-                                              _ptr(res), _ptr(res2), _ptr(mask), _ptr(y), _ptr(ws), ws.numel() * 4 if ws is not None else 0,
-                                              _stream()), 'dvd_conv2d_nhwc_ws')
+                                              _ptr(res), _ptr(res2), _ptr(mask), _ptr(y), _ptr(workspace), ws_bytes, _stream()),
+               'dvd_conv2d_nhwc_ws')
     if ev is not None:
         ev.record()
     return y
@@ -379,16 +370,19 @@ class Conv:
         d = make_desc(N, H, W, self.cin, OH, OW, self.cout, fwd_taps(self.k, self.pad), self.stride, self.kblock, relu=relu,
                       round_out=round_out, bn_eps=self.bn.eps if self.bn is not None else 0.0)
         y = empty_cl(N, self.cout, OH, OW, x.device)
-        return conv2d_launch(d, x, self.w_fwd, y, self.conv.bias, self._bn_fwd(), res, res2, flops=self.flops(N, OH, OW), kind='fwd')
+        return conv2d_launch(d, x, self.w_fwd, y, self.conv.bias, self._bn_fwd(), res, res2, flops=self.flops(N, OH, OW), kind='fwd',
+                             workspace=conv_workspace(x.device))
 
     # -- data gradient: gx = [mask > 0] * (conv^T(gy) + res + res2);  gy must be the gradient w.r.t. the convolution's
     #    BatchNorm OUTPUT (the scale is folded into the weight image) -------------------------------------------------
     def dgrad(self, gy, H, W, res=None, res2=None, mask=None, round_out=True):
         N, Co, OH, OW = gy.shape
         gx = empty_cl(N, self.cin, H, W, gy.device)
+        ws = conv_workspace(gy.device)
         if self.stride == 1:
             d = make_desc(N, OH, OW, self.cout, H, W, self.cin, dgrad_taps_s1(self.k, self.pad), 1, self.kblock, round_out=round_out)
-            return conv2d_launch(d, gy, self.w_bwd, gx, res=res, res2=res2, mask=mask, flops=self.flops(N, OH, OW), kind='dgrad')
+            return conv2d_launch(d, gy, self.w_bwd, gx, res=res, res2=res2, mask=mask, flops=self.flops(N, OH, OW), kind='dgrad',
+                                 workspace=ws)
         phases = [(a, b, dgrad_phase_taps_s2(self.k, self.pad, a, b)) for a in (0, 1) for b in (0, 1)]
         if any(not t for _, _, t in phases):
             if res is not None or res2 is not None or mask is not None:
@@ -403,7 +397,7 @@ class Conv:
             d = make_desc(N, OH, OW, self.cout, ph, pw, self.cin, taps, 1, self.kblock, YH=H, YW=W, out_map=(2, a, 2, b),
                           round_out=round_out)
             conv2d_launch(d, gy, self.w_bwd, gx, res=res, res2=res2, mask=mask, kind='dgrad',
-                          flops=self.flops(N, OH, OW) * len(taps) / (self.k * self.k))
+                          flops=self.flops(N, OH, OW) * len(taps) / (self.k * self.k), workspace=ws)
         return gx
 
     # -- weight gradient (accumulates into conv.weight.grad; BatchNorm: gy un-scaled, dgamma gets the <W, dW> term). With

@@ -717,27 +717,27 @@ int per_device_attr(const void* func, size_t smem_bytes, bool (&done)[16]) {
   return 0;
 }
 
-// how many clusters of `csize` CTAs of this kernel can be resident at once (cached per device and size)
+// how many CTAs of this kernel can be resident at once (cached per device)
 template <typename K>
-int max_clusters(K kernel, int threads, size_t smem_bytes, int csize) {
-  static int cache[16][5] = {};
+int resident_ctas(K kernel, int threads, size_t smem_bytes) {
+  static int cache[16] = {};
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 16) dev = 0;
-  if (cache[dev][csize] > 0) return cache[dev][csize];
+  if (cache[dev] > 0) return cache[dev];
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(num_sms() / csize * csize));
+  cfg.gridDim = dim3((unsigned)num_sms());
   cfg.blockDim = dim3((unsigned)threads);
   cfg.dynamicSmemBytes = smem_bytes;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = (unsigned)csize;
+  attr[0].val.clusterDim.x = 1;
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   int n = 0;
-  if (cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) != cudaSuccess || n < 1) n = num_sms() / csize;
-  cache[dev][csize] = n;
+  if (cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) != cudaSuccess || n < 1) n = num_sms();
+  cache[dev] = n;
   return n;
 }
 
@@ -755,7 +755,7 @@ int launch_wgrad(const CUtensorMap& mapM, const CUtensorMap& mapN, WgradParams P
   static bool attr_done[16] = {};
   if (int e = per_device_attr((const void*)conv_wgrad_kernel<NT, G64>, kWgSmem, attr_done)) return e;
   // split-K so that all CTAs are resident in ONE wave (a second, nearly empty wave would double the time)
-  const int resident = max_clusters(conv_wgrad_kernel<NT, G64>, kWgThreads, kWgSmem, 1);
+  const int resident = resident_ctas(conv_wgrad_kernel<NT, G64>, kWgThreads, kWgSmem);
   int ksplit = resident / out_tiles;
   if (ksplit > px_tiles) ksplit = px_tiles;
   if (ksplit < 1) ksplit = 1;
@@ -852,8 +852,7 @@ extern "C" int dvd_conv2d_nhwc_ws(const dvd_conv_desc* desc, const float* x, con
       const long waves0 = (tiles0 + full - 1) / full, total0 = tiles0 * ksteps, mu = ksteps / 4 > 8 ? ksteps / 4 : 8;
       long nc0 = total0 / mu;
       if (nc0 > full) nc0 = full;
-      const char* evs = getenv("DVD_CONV_STREAMK");
-      if (workspace && ksteps >= 8 && !(evs && atoi(evs) == 0) && nc0 >= 1 && waves0 * ksteps - (total0 + nc0 - 1) / nc0 >= 64)
+      if (workspace && ksteps >= 8 && nc0 >= 1 && waves0 * ksteps - (total0 + nc0 - 1) / nc0 >= 64)
         nt_min = nt_max;
       double best = 1e30;
       for (int nt = nt_max; nt >= nt_min; nt -= 32) {
@@ -890,9 +889,7 @@ extern "C" int dvd_conv2d_nhwc_ws(const dvd_conv_desc* desc, const float* x, con
     const long ksteps = (long)d.ntaps * P.kchunks, total = ctiles * ksteps;
     const long waves = (ctiles + full - 1) / full;
     const double eff = (double)ctiles / (double)(waves * full);
-    const char* ev = getenv("DVD_CONV_STREAMK");
-    const bool allowed = !(ev && atoi(ev) == 0);
-    if (allowed && workspace && ksteps >= 8 && eff < 0.88) {
+    if (workspace && ksteps >= 8 && eff < 0.88) {
       const long min_units = ksteps / 4 > 8 ? ksteps / 4 : 8;
       long nc = total / min_units;
       if (nc > full) nc = full;
@@ -1027,18 +1024,4 @@ extern "C" int dvd_conv2d_wgrad(const dvd_conv_desc* desc, const float* x, const
     case 224: return launch_wgrad<224, false>(mapM, mapN, P, out_tiles, px_tiles, st);
     default: return launch_wgrad<256, false>(mapM, mapN, P, out_tiles, px_tiles, st);
   }
-}
-
-/* resident CTAs of the two tensor-core kernels for cluster sizes 1, 2, 4 (diagnostic): out[0..2] forward / data gradient kernel,
- * out[3..5] weight-gradient kernel */
-extern "C" int dvd_conv2d_cluster_info(int* out) {
-  static bool a1[16] = {}, a2[16] = {};
-  if (int e = per_device_attr((const void*)conv2d_tc_kernel<kMaxNT>, kSmem, a1)) return e;
-  if (int e = per_device_attr((const void*)conv_wgrad_kernel<256, false>, kWgSmem, a2)) return e;
-  const int cs[3] = {1, 2, 4};
-  for (int i = 0; i < 3; ++i) {
-    out[i] = cs[i] * max_clusters(conv2d_tc_kernel<kMaxNT>, kThreads, kSmem, cs[i]);
-    out[3 + i] = cs[i] * max_clusters(conv_wgrad_kernel<256, false>, kWgThreads, kWgSmem, cs[i]);
-  }
-  return 0;
 }

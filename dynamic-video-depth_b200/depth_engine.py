@@ -59,97 +59,42 @@ class MidasEngine:
         self.oc0, self.oc2, self.oc4 = Conv(s.output_conv[0]), Conv(s.output_conv[2]), s.output_conv[4]
         self._all = [c for st in self.stages for b in st for c in b.convs()] + self.rn
         self._all += [c for r in self.rcu_a[:3] + self.rcu_b for c in (r.c1, r.c2)] + [self.oc0, self.oc2]
-        self.saved = None
+        self.saved = None           # what backward() needs, kept by a training forward
         self._table = None
-        self._lane, self._lane_pool, self._lanes, self._n_active_lanes = None, {}, None, 1
+        self._sides = {}            # device index -> side stream of the two-stream backward
+        self._side = None           # the side stream of the backward in progress
+        self._keep = []
         # called as grad_hook(stage) at the points of backward() where a contiguous block of parameter gradients is final:
         # 'decoder+layer4', 'layer3', 'rest' - the data-parallel path all-reduces that block while the backward goes on
         self.grad_hook = None
 
     # ---------------------------------------------------------------------------------------------------
-    # Streams. (1) Two-stream backward: the weight gradient of a layer depends only on tensors the data-gradient chain has already
-    # produced (the layer's input activation and the masked gradient of its output): it is issued on a SIDE stream behind an event,
-    # while the lane's main stream goes on with the data gradient. Both kernels are persistent one-CTA-per-SM grids, so the hardware
-    # fills the SMs a finishing grid leaves idle (its last, partly empty wave; launch latency; prologue) with CTAs of the other
-    # stream. Tensors handed to the side stream are kept alive until the next join (the caching allocator would otherwise hand
-    # their memory to the main stream while the side stream still reads it).
-    # (2) Lanes (opt-in, DVD_LANES=2): the images can be split into two independent LANES (own stream, own side stream, own
-    # stream-K exchange area) whose kernels run side by side on disjoint SMs. A lane keeps its streams from forward to backward,
-    # so every tensor is allocated, used and freed in one stream order. Not the default: see _lanes_for.
-    class _Lane:
-        def __init__(self, index, stream, side):
-            self.index, self.stream, self.side = index, stream, side
-            self.keep, self.saved = [], None
-
-    def _lanes_for(self, n_images):
-        # opt-in (DVD_LANES=2): splitting doubles the number of launches, and what a launch costs at these sizes is its fixed
-        # part, so two half-size chains side by side only break even on that
-        want = 2 if (os.environ.get('DVD_LANES', '') == '2' and n_images % 2 == 0 and n_images >= 2) else 1
-        dev = torch.cuda.current_device()
-        pool = self._lane_pool.setdefault(dev, [])
-        while len(pool) < want:
-            i = len(pool)
-            pool.append(MidasEngine._Lane(i, None if i == 0 else torch.cuda.Stream(device=dev), torch.cuda.Stream(device=dev)))
-        return pool[:want]
-
-    def _in_lane(self, lane):
-        """context: kernels go to the lane's stream, stream-K launches use the lane's exchange area"""
-        eng = self
-
-        class _Ctx:
-            def __enter__(self_):
-                self_.prev = eng._lane
-                eng._lane = lane
-                # one lane: its own exchange area (stream-K allowed); several concurrent lanes: none (see set_workspace_lane)
-                self_.prev_ws = co.set_workspace_lane(lane.index if eng._n_active_lanes == 1 else -1)
-                self_.sc = torch.cuda.stream(lane.stream) if lane.stream is not None else None
-                if self_.sc is not None:
-                    self_.sc.__enter__()
-
-            def __exit__(self_, *a):
-                if self_.sc is not None:
-                    self_.sc.__exit__(*a)
-                co.set_workspace_lane(self_.prev_ws)
-                eng._lane = self_.prev
-        return _Ctx()
-
-    @staticmethod
-    def _fork(lanes):
-        """every lane's stream (and nothing else) waits for what the current stream has enqueued so far"""
-        ev = torch.cuda.Event()
-        ev.record()
-        for ln in lanes:
-            if ln.stream is not None:
-                ln.stream.wait_event(ev)
-
-    @staticmethod
-    def _join(lanes):
-        for ln in lanes:
-            if ln.stream is not None:
-                ev = torch.cuda.Event()
-                ev.record(ln.stream)
-                torch.cuda.current_stream().wait_event(ev)
-
+    # Two-stream backward: the weight gradient of a layer depends only on tensors the data-gradient chain has already produced
+    # (the layer's input activation and the masked gradient of its output): it is issued on a SIDE stream behind an event, while
+    # the main stream goes on with the data gradient. Both kernels are persistent one-CTA-per-SM grids, so the hardware fills the
+    # SMs a finishing grid leaves idle (its last, partly empty wave; launch latency; prologue) with CTAs of the other stream.
+    # Tensors handed to the side stream are kept alive until the next join (the caching allocator would otherwise hand their
+    # memory to the main stream while the side stream still reads it). The weight-gradient launches take no stream-K exchange
+    # area, so the data-gradient launches on the main stream keep theirs to themselves.
     def _on_side(self, fn, *keep):
-        ln = self._lane
-        if ln is None or ln.side is None or os.environ.get('DVD_BWD_OVERLAP', '1') == '0':
+        if os.environ.get('DVD_BWD_OVERLAP', '1') == '0':
             fn()
             return
         ev = torch.cuda.Event()
         ev.record()
-        ln.side.wait_event(ev)
-        with torch.cuda.stream(ln.side):
+        self._side.wait_event(ev)
+        with torch.cuda.stream(self._side):
             fn()
-        ln.keep.extend(keep)
+        self._keep.extend(keep)
 
-    def _side_join(self):
-        ln = self._lane
-        if ln is None or ln.side is None:
-            return
+    def _stage_done(self, stage):
+        """the parameter gradients of `stage` are final once the main stream has joined the side stream: hand them to grad_hook"""
         ev = torch.cuda.Event()
-        ev.record(ln.side)
+        ev.record(self._side)
         torch.cuda.current_stream().wait_event(ev)
-        ln.keep.clear()
+        self._keep.clear()
+        if self.grad_hook is not None:
+            self.grad_hook(stage)
 
     # ---------------------------------------------------------------------------------------------------
     def pack(self, need_bwd=True):
@@ -167,25 +112,6 @@ class MidasEngine:
         """x [N,3,H,W] raw image in [0,1] (contiguous fp32 CUDA) -> depth [N,1,H,W]. train=True keeps what backward needs."""
         self.pack(need_bwd=train)
         x = x.contiguous()
-        lanes = self._lanes_for(x.shape[0])
-        self._n_active_lanes = len(lanes)
-        if len(lanes) == 1:
-            with self._in_lane(lanes[0]):
-                depth, lanes[0].saved = self._forward_one(x, train)
-        else:
-            depth = torch.empty((x.shape[0], 1) + tuple(x.shape[2:]), dtype=torch.float32, device=x.device)
-            per = x.shape[0] // len(lanes)
-            self._fork(lanes)
-            for i, ln in enumerate(lanes):
-                with self._in_lane(ln):
-                    d, ln.saved = self._forward_one(x[i * per:(i + 1) * per], train)
-                    depth[i * per:(i + 1) * per].copy_(d)
-            self._join(lanes)
-        self._lanes = lanes if train else None
-        self.saved = True if train else None
-        return depth
-
-    def _forward_one(self, x, train):
         nm, ns = (_NORM_MEAN, _NORM_STD) if self.normalize else (None, None)
         a0 = co.stem_fwd(x, self.stem_conv, self.stem_bn, nm, ns)
         a1, pool_idx = co.maxpool_fwd(a0)
@@ -225,50 +151,21 @@ class MidasEngine:
         depth = co.head_fwd(h2, self.oc4.weight, self.oc4.bias)
         if train:
             S.update(feats=feats, lr=lr, dec=dec, p1=path, h1=h1, h2=h2)
-        return depth, S
+        self.saved = S
+        return depth
 
     # ---------------------------------------------------------------------------------------------------
     def backward(self, g_depth):
         """Accumulates dL/dparam into .grad for every parameter of the net, given dL/ddepth [N,1,H,W]."""
-        lanes = self._lanes
-        if self.saved is None or lanes is None:
+        S, self.saved = self.saved, None
+        if S is None:
             raise RuntimeError('MidasEngine.backward without a training forward')
-        self.saved, self._lanes = None, None
-        self._n_active_lanes = len(lanes)
         self._ensure_grads()
         g_depth = g_depth.contiguous()
-        per = g_depth.shape[0] // len(lanes)
-        gens = [self._backward_gen(ln.saved, g_depth[i * per:(i + 1) * per]) for i, ln in enumerate(lanes)]
-        for ln in lanes:
-            ln.saved = None
-        self._fork(lanes)
-        # the lanes advance stage by stage (host order = lane 0, lane 1, ... within a stage): a block of parameter gradients is
-        # final - and handed to the gradient exchange - when every lane has passed it
-        nm, ns = (_NORM_MEAN, _NORM_STD) if self.normalize else (None, None)
-        stem = []
-        for stage in ('decoder+layer4', 'layer3', 'pre-stem'):
-            for ln, gen in zip(lanes, gens):
-                with self._in_lane(ln):
-                    out = next(gen)
-                    assert out[0] == stage
-                    if stage == 'pre-stem':
-                        if len(lanes) == 1:      # (while the last weight gradients are still running on the side stream)
-                            co.stem_wgrad(*out[1], self.stem_conv, self.stem_bn, nm, ns)
-                        else:
-                            stem.append(out[1])
-                    self._side_join()
-            self._join(lanes)
-            if stage != 'pre-stem' and self.grad_hook is not None:
-                self.grad_hook(stage)
-        # several lanes: the stem's weight-gradient finalisation is a plain read-modify-write of the 3 -> 64 filter, so one lane
-        # after the other on the main stream
-        for xs, g_a0, a0 in stem:
-            co.stem_wgrad(xs, g_a0, a0, self.stem_conv, self.stem_bn, nm, ns)
-        if self.grad_hook is not None:
-            self.grad_hook('rest')
-
-    def _backward_gen(self, S, g_depth):
-        """one lane's backward as a generator: yields at the points where a contiguous block of parameter gradients is complete"""
+        dev = torch.cuda.current_device()
+        if dev not in self._sides:
+            self._sides[dev] = torch.cuda.Stream(device=dev)
+        self._side = self._sides[dev]
         oc4 = self.oc4
         gm_h2 = co.head_bwd(S['h2'], oc4.weight, oc4.bias, g_depth, oc4.weight.grad, oc4.bias.grad, relu_mask=True)
         H1, W1 = S['h1'].shape[2:]
@@ -328,10 +225,13 @@ class MidasEngine:
                     g_in = b.c1.dgrad(gm1, Hi, Wi, res=gm3, res2=extra, mask=x_in)
                 gm3 = g_in
             if si in (3, 2):
-                yield ('decoder+layer4' if si == 3 else 'layer3',)
+                self._stage_done('decoder+layer4' if si == 3 else 'layer3')
         a0 = S['a0']
         g_a0 = co.maxpool_bwd(g_in, S['pool_idx'], a0.shape[2], a0.shape[3])
-        yield ('pre-stem', (S['x'], g_a0, a0))
+        # issued while the last weight gradients are still running on the side stream
+        nm, ns = (_NORM_MEAN, _NORM_STD) if self.normalize else (None, None)
+        co.stem_wgrad(S['x'], g_a0, a0, self.stem_conv, self.stem_bn, nm, ns)
+        self._stage_done('rest')
 
 
 class MidasFunction(torch.autograd.Function):

@@ -110,7 +110,7 @@ def _raft(name, *args):
 
 class _TC:
     """One dvd_conv2d_nhwc launch: weight [Cout,Cin,kh,kw] packed once (TF32-rounded, tap-major), bias and eval BatchNorm in
-    the epilogue."""
+    the epilogue. It passes no exchange area, so the launch runs whole tiles only."""
 
     def __init__(self, weight, bias, stride=1, padding=(0, 0), bn=None, relu=False, round_out=True):
         weight = weight.detach()
@@ -338,45 +338,41 @@ class RaftNet(nn.Module):
         a copy of every intermediate tensor under the names of oracle/raft_tf32.py (NHWC)"""
         images = self._check_images(images)
         P = self.plan()
-        prev = conv_ops.set_workspace_lane(-1)
-        try:
-            x = self.feature_stem(images, trace)
-            _keep(trace, 'fnet.stem.out', x)
-            for name, (c1, c2, ds) in zip(BLOCK_NAMES, P.f_blocks):
-                p = 'fnet.' + name + '.'
-                a = c1(x)
-                y = norm_act(a, instnorm_stats(a), relu_inner=True)
-                b = c2(y)
-                _keep(trace, p + 'a', a)
-                _keep(trace, p + 'y', y)
-                _keep(trace, p + 'b', b)
-                if ds is None:
-                    x = norm_act(b, instnorm_stats(b), res=x, relu_inner=True, relu_outer=True)
-                else:
-                    yb = norm_act(b, instnorm_stats(b), relu_inner=True, round_out=False)
-                    d = ds(x)
-                    x = norm_act(d, instnorm_stats(d), res=yb, relu_outer=True)
-                    _keep(trace, p + 'yb', yb)
-                    _keep(trace, p + 'd', d)
-                _keep(trace, p + 'out', x)
-            fmap = P.f_out(x)
-            _keep(trace, 'fmap', fmap)
-            x = self.context_stem(images)
-            _keep(trace, 'cnet.stem.out', x)
-            for name, (c1, c2, ds) in zip(BLOCK_NAMES, P.c_blocks):
-                p = 'cnet.' + name + '.'
-                y = c1(x)
-                b = c2(y)
-                # relu(x + relu(bn2(conv2))): the shortcut is added after the branch's own ReLU, so it is not the convolution's residual
-                x = norm_act(b, res=x, relu_outer=True) if ds is None else ds(x, res=b)
-                _keep(trace, p + 'y', y)
-                _keep(trace, p + 'b', b)
-                _keep(trace, p + 'out', x)
-            cnet = P.c_out(x)
-            _keep(trace, 'cnet', cnet)
-            return FrameFeatures(fmap, cnet)
-        finally:
-            conv_ops.set_workspace_lane(prev)
+        x = self.feature_stem(images, trace)
+        _keep(trace, 'fnet.stem.out', x)
+        for name, (c1, c2, ds) in zip(BLOCK_NAMES, P.f_blocks):
+            p = 'fnet.' + name + '.'
+            a = c1(x)
+            y = norm_act(a, instnorm_stats(a), relu_inner=True)
+            b = c2(y)
+            _keep(trace, p + 'a', a)
+            _keep(trace, p + 'y', y)
+            _keep(trace, p + 'b', b)
+            if ds is None:
+                x = norm_act(b, instnorm_stats(b), res=x, relu_inner=True, relu_outer=True)
+            else:
+                yb = norm_act(b, instnorm_stats(b), relu_inner=True, round_out=False)
+                d = ds(x)
+                x = norm_act(d, instnorm_stats(d), res=yb, relu_outer=True)
+                _keep(trace, p + 'yb', yb)
+                _keep(trace, p + 'd', d)
+            _keep(trace, p + 'out', x)
+        fmap = P.f_out(x)
+        _keep(trace, 'fmap', fmap)
+        x = self.context_stem(images)
+        _keep(trace, 'cnet.stem.out', x)
+        for name, (c1, c2, ds) in zip(BLOCK_NAMES, P.c_blocks):
+            p = 'cnet.' + name + '.'
+            y = c1(x)
+            b = c2(y)
+            # relu(x + relu(bn2(conv2))): the shortcut is added after the branch's own ReLU, so it is not the convolution's residual
+            x = norm_act(b, res=x, relu_outer=True) if ds is None else ds(x, res=b)
+            _keep(trace, p + 'y', y)
+            _keep(trace, p + 'b', b)
+            _keep(trace, p + 'out', x)
+        cnet = P.c_out(x)
+        _keep(trace, 'cnet', cnet)
+        return FrameFeatures(fmap, cnet)
 
     # -- update iterations ----------------------------------------------------------------------------
     def update_step(self, P, pyr, coords1, net, X, XR, net_r, want_delta=False, trace=None):
@@ -447,25 +443,21 @@ class RaftNet(nn.Module):
         if len(feat_a) != len(feat_b) or feat_a.fmap.shape != feat_b.fmap.shape:
             raise ValueError('feat_a and feat_b must hold the same number of frames of one size')
         P = self.plan()
-        prev = conv_ops.set_workspace_lane(-1)
-        try:
-            fa, fb, cn = feat_a.fmap.contiguous(), feat_b.fmap.contiguous(), feat_a.cnet.contiguous()
-            B, h, w, _ = fa.shape
-            pyr = corr_pyramid(fa, fb)
-            _keep(trace, 'pyramid', pyr)
-            net, X, XR, net_r = self.init_state(cn, trace)
-            coords1 = coords_grid(B, h, w, fa.device)
-            for _ in range(iters):
-                it = None
-                if trace is not None:
-                    it = {}
-                    trace.setdefault('iters', []).append(it)
-                self.update_step(P, pyr, coords1, net, X, XR, net_r, trace=it)
-            up = upsample(self.mask_parts(P, net_r, trace), coords1)
-            _keep(trace, 'flow_up', up)
-            return (up, coords1 - coords_grid(B, h, w, fa.device)) if return_low else up
-        finally:
-            conv_ops.set_workspace_lane(prev)
+        fa, fb, cn = feat_a.fmap.contiguous(), feat_b.fmap.contiguous(), feat_a.cnet.contiguous()
+        B, h, w, _ = fa.shape
+        pyr = corr_pyramid(fa, fb)
+        _keep(trace, 'pyramid', pyr)
+        net, X, XR, net_r = self.init_state(cn, trace)
+        coords1 = coords_grid(B, h, w, fa.device)
+        for _ in range(iters):
+            it = None
+            if trace is not None:
+                it = {}
+                trace.setdefault('iters', []).append(it)
+            self.update_step(P, pyr, coords1, net, X, XR, net_r, trace=it)
+        up = upsample(self.mask_parts(P, net_r, trace), coords1)
+        _keep(trace, 'flow_up', up)
+        return (up, coords1 - coords_grid(B, h, w, fa.device)) if return_low else up
 
     def forward(self, image1, image2, iters=20, flow_init=None, upsample=True, test_mode=True):
         """RAFT.forward(image1, image2, iters, test_mode=True) -> (flow_low [B,2,H/8,W/8], flow_up [B,2,H,W])"""

@@ -284,9 +284,6 @@ int dvd_conv2d_wgrad(const dvd_conv_desc* desc, const float* x, const float* gy,
                      long stride_co, long stride_ci, long stride_ky, long stride_kx, int ksize, int groups,
                      const float* bn_gamma, const float* bn_var, float* dgamma, float* colsum, const float* bn_mean,
                      void* stream);
-/* diagnostic: CTAs of the two tensor-core kernels that can be resident at once when launched in thread-block clusters of 1, 2, 4
- * (out[0..2] dvd_conv2d_nhwc, out[3..5] dvd_conv2d_wgrad): the library picks the cluster size that keeps the machine full.  */
-int dvd_conv2d_cluster_info(int* out6);
 
 /* ---- CUDA-core members of the MiDaS path (csrc/depth_ops.cu), NHWC fp32 -------------------------------------------------- */
 /* y = round-to-nearest TF32 of x (n % 4 == 0): entry of foreign tensors into the rounded-operand contract                   */

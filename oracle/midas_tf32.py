@@ -181,7 +181,7 @@ def anchor_names(n_blocks=33):
 
 
 def engine_anchors(S):
-    """a lane's saved dict of MidasEngine._forward_one -> {anchor name: tensor}"""
+    """MidasEngine.saved (what a training forward keeps for the backward) -> {anchor name: tensor}"""
     A = {'a0': S['a0'], 'pool_idx': S['pool_idx']}
     for bi, (cur, y1, y2) in enumerate(S['blocks']):
         A['block%d.cur' % bi], A['block%d.y1' % bi], A['block%d.y2' % bi] = cur, y1, y2

@@ -115,7 +115,8 @@ def test_conv_forward_matches_torch_fp64(case):
         if not has_mask else None
     if has_mask:
         d = co.make_desc(N, H, W, ci, OH, OW, co_, co.fwd_taps(k, k // 2), stride, c.kblock, relu=relu, round_out=False)
-        y = co.conv2d_launch(d, cl(x), c.w_fwd, co.empty_cl(N, co_, OH, OW, 'cuda'), conv.bias, None, None, None, cl(mask))
+        y = co.conv2d_launch(d, cl(x), c.w_fwd, co.empty_cl(N, co_, OH, OW, 'cuda'), conv.bias, None, None, None, cl(mask),
+                             workspace=co.conv_workspace(torch.device('cuda')))
     assert y.shape == ref.shape and y.is_contiguous(memory_format=torch.channels_last)
     e = rel_err(y, ref)
     assert e < TOL, e
@@ -125,11 +126,10 @@ def test_conv_forward_matches_torch_fp64(case):
         assert torch.equal(y2, co.round_tf32(y))
 
 
-def test_stream_k_schedule_matches_whole_tiles_and_leaves_flags_clear():
-    """Same launch with and without the stream-K schedule (DVD_CONV_STREAMK=0 = whole tiles): equal up to fp32 summation order;
+def test_stream_k_matches_a_launch_without_workspace_and_leaves_flags_clear():
+    """Same launch with and without the stream-K schedule (no exchange area = whole tiles): equal up to fp32 summation order;
     the flag words of the exchange area are back to zero afterwards (the next launch relies on it); launches of OTHER shapes in
     between (other tile widths, cluster counts) must not disturb it (stale lines of the exchange area in an SM's L1 did, once)."""
-    import os
     from dvd_b200 import conv_ops as co
     g = gen(77)
 
@@ -145,14 +145,13 @@ def test_stream_k_schedule_matches_whole_tiles_and_leaves_flags_clear():
     assert ws is not None
     ws[256:].zero_()
     ref = []
-    os.environ['DVD_CONV_STREAMK'] = '0'
-    try:
-        for c, x in layers:
-            ref.append(c.fwd(x, relu=True, round_out=False))
-        torch.cuda.synchronize()
-        assert float(ws[256:].abs().max()) == 0.0
-    finally:
-        del os.environ['DVD_CONV_STREAMK']
+    for c, x in layers:
+        N, _, H, W = x.shape
+        OH, OW = c.out_hw(H, W)
+        d = co.make_desc(N, H, W, c.cin, OH, OW, c.cout, co.fwd_taps(c.k, c.pad), relu=True, round_out=False)
+        ref.append(co.conv2d_launch(d, x, c.w_fwd, co.empty_cl(N, c.cout, OH, OW, 'cuda'), c.conv.bias, workspace=None))
+    torch.cuda.synchronize()
+    assert float(ws[256:].abs().max()) == 0.0
     first = None
     for rep in range(3):
         outs = [c.fwd(x, relu=True, round_out=False) for c, x in layers]

@@ -102,18 +102,6 @@ def _cotangent(kind, N, H, W):
     return (1e-3 * (1 + 0.5 * torch.sin(9.0 * yy + ph) * torch.cos(7.0 * xx - ph))).cuda()
 
 
-def _merge_lanes(saved):
-    if len(saved) == 1:
-        return saved[0]
-    cat = lambda ts: None if ts[0] is None else torch.cat(ts, 0)
-    S = {k: cat([s[k] for s in saved]) for k in ('x', 'a0', 'pool_idx', 'p1', 'h1', 'h2')}
-    for k in ('blocks', 'dec'):
-        S[k] = [tuple(cat(list(z)) for z in zip(*tup)) for tup in zip(*[s[k] for s in saved])]
-    for k in ('feats', 'lr'):
-        S[k] = [cat(list(z)) for z in zip(*[s[k] for s in saved])]
-    return S
-
-
 def _check_engine_against_emulation(N, H, W, kind):
     from oracle.midas_tf32 import Anchors, anchor_names, engine_anchors, midas_tf32_forward
     net = _net()
@@ -124,7 +112,7 @@ def _check_engine_against_emulation(N, H, W, kind):
     for p in net.parameters():
         p.grad = None
     depth = eng.forward(x, train=True)
-    S = _merge_lanes([ln.saved for ln in eng._lanes])
+    S = eng.saved
     eng.backward(cot)
     A = engine_anchors(S)
     bi = 0
@@ -189,25 +177,19 @@ def _check_engine_against_emulation(N, H, W, kind):
 
 @pytest.mark.parametrize('kind', ['smooth', 'white'])
 @pytest.mark.parametrize('shape', [(2, 64, 96), (1, 224, 384)])
-def test_engine_matches_tf32_emulation(shape, kind, monkeypatch):
-    for k in ('DVD_BWD_OVERLAP', 'DVD_LANES'):
-        monkeypatch.delenv(k, raising=False)
+def test_saved_tensors_match_tf32_emulation(shape, kind, monkeypatch):
+    monkeypatch.delenv('DVD_BWD_OVERLAP', raising=False)
     _check_engine_against_emulation(*shape, kind)
 
 
-@pytest.mark.parametrize('env', [{'DVD_BWD_OVERLAP': '0'}, {'DVD_LANES': '2'}], ids=['one_stream', 'two_lanes'])
-def test_stream_schedules_match_tf32_emulation(env, monkeypatch):
-    for k in ('DVD_BWD_OVERLAP', 'DVD_LANES'):
-        monkeypatch.delenv(k, raising=False)
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
+def test_one_stream_backward_matches_tf32_emulation(monkeypatch):
+    monkeypatch.setenv('DVD_BWD_OVERLAP', '0')
     _check_engine_against_emulation(4, 64, 96, 'white')
 
 
 @pytest.mark.timeout(1200)
-def test_engine_matches_tf32_emulation_at_bench_resolution(monkeypatch):
+def test_saved_tensors_match_tf32_emulation_at_bench_resolution(monkeypatch):
     """the bench resolution at a bench-like batch, so the layers run the tile shapes and schedules (stream-K among them) of a
     training step. 8 images rather than the bench's 16: the fp64 emulation with its autograd graph needs about 2.2 GB per image at 224 x 384 (17-19 GB at 8)."""
-    for k in ('DVD_BWD_OVERLAP', 'DVD_LANES'):
-        monkeypatch.delenv(k, raising=False)
+    monkeypatch.delenv('DVD_BWD_OVERLAP', raising=False)
     _check_engine_against_emulation(8, 224, 384, 'white')

@@ -210,7 +210,7 @@ def gru_state(net_in, inp):
 
 
 @pytest.mark.parametrize('it', [0, 3])
-def test_one_update_iteration_from_the_fixture_state(gold, sd, net, it):
+def test_update_step_alone_from_the_fixture_state(gold, sd, net, it):
     from oracle import raft as oracle_raft
     case = gold['cases'][0]
     sdg = oracle_raft.cast(sd, torch.float32, 'cuda')
@@ -219,12 +219,7 @@ def test_one_update_iteration_from_the_fixture_state(gold, sd, net, it):
     hidden, X, XR, net_r = gru_state(st['net_in'], case['inp'])
     coords1 = nhwc(case['coords1'][it:it + 1]).cuda()
     before = coords1.clone()
-    from dvd_b200 import conv_ops
-    prev = conv_ops.set_workspace_lane(-1)
-    try:
-        _, delta = net.update_step(net.plan(), pyr, coords1, hidden, X, XR, net_r, want_delta=True)
-    finally:
-        conv_ops.set_workspace_lane(prev)
+    _, delta = net.update_step(net.plan(), pyr, coords1, hidden, X, XR, net_r, want_delta=True)
     e = {'net': rel(nchw(hidden), st['net']), 'delta_flow': rel(nchw(delta), case['delta_flow'][it:it + 1])}
     flow = case['coords1'][it:it + 1] - oracle_raft.coords_grid(1, *case['coords1'].shape[-2:], torch.float32, 'cpu')
     r_net, r_delta = eager_tf32(lambda: oracle_raft.update(sdg, st['net_in'].cuda(), case['inp'].cuda(), st['corr'].cuda(), flow.cuda()))

@@ -75,10 +75,7 @@ def main():
         pyr = raft.corr_pyramid(fa.fmap, fb.fmap)
         state = net.init_state(fa.cnet)
         coords1 = raft.coords_grid(B, h, w, 'cuda')
-        from dvd_b200 import conv_ops
-        prev = conv_ops.set_workspace_lane(-1)
         t = timed(lambda: net.update_step(P, pyr, coords1, *state), 20)
-        conv_ops.set_workspace_lane(prev)
         fl = iteration_flops(P, B * npx)
         res['update_iteration_B%d' % B] = {'s': t, 's_per_pair': t / B, 'GFLOP_per_pair': fl / B / 1e9, 'TFLOP_per_s': fl / t / 1e12}
 

@@ -15,11 +15,6 @@ def main():
     from dvd_b200 import conv_ops, synthetic
     from dvd_b200.third_party.MiDaS import MidasNet
     tag = sys.argv[1] if len(sys.argv) > 1 else 'r2'
-    import ctypes
-    from dvd_b200 import _lib
-    info = (ctypes.c_int * 6)()
-    _lib.check(_lib.load().dvd_conv2d_cluster_info(info), 'cluster_info')
-    print('resident CTAs at cluster size 1/2/4: conv', list(info)[:3], 'wgrad', list(info)[3:])
     N = int(os.environ.get('IMAGES', '16'))
     net = synthetic.seed_net_(MidasNet(non_negative=True, normalize_input=True), 0, 2000.0).eval().cuda()
     x = torch.rand(N, 3, 224, 384, device='cuda')
