@@ -128,6 +128,8 @@ SIGNATURES = {
     'dvd_calib_ratios': [_P, _P, ctypes.c_size_t, _P, _P, ctypes.c_long, ctypes.c_double, ctypes.c_double, ctypes.c_double,
                          ctypes.c_double, _P, ctypes.c_size_t, _I, _I, _I, _P],
     'dvd_sorted_median': [_P, ctypes.c_size_t, _I, ctypes.c_long, _P, _P, _P],
+    'dvd_sorted_median_f32': [_P, ctypes.c_size_t, _I, ctypes.c_long, _P, _P, _P],
+    'dvd_dense_ratios': [_P, ctypes.c_size_t, _P, ctypes.c_size_t, _I, _P, ctypes.c_size_t, _I, ctypes.c_long, _P],
     'dvd_aa_resize_scratch_bytes': [_I, _I, _I, _I],
     'dvd_aa_resize': [_P, ctypes.c_size_t, _P, ctypes.c_size_t, _P, ctypes.c_size_t, _P, _I, _P, _I, _I, _I, _I, _I, _I, _I, _P],
 }

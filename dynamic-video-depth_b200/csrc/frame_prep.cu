@@ -1,11 +1,13 @@
-// Frame preparation: the GPU side of scripts/preprocess/davis/generate_frame_midas.py. MiDaS's bicubic resizes around the
-// depth engine, scipy's order-3 spline (prefilter + sampling, mode 'constant') for the scale calibration's point selection
-// and depth look-up, the per-frame median of nn / depth, and skimage's anti-aliased resize (gaussian_filter, then
-// zoom(order=1, mode='mirror', grid_mode=True), then clip) for the working-size outputs.
+// Frame preparation: the GPU side of scripts/preprocess/{davis,shutterstock}/generate_frame_midas.py. MiDaS's bicubic resizes
+// around the depth engine, scipy's order-3 spline (prefilter + sampling, mode 'constant') for the DAVIS scale calibration's
+// point selection and depth look-up, the ShutterStock calibration's dense per-pixel ratios, the per-frame median of the
+// ratios, and skimage's anti-aliased resize (gaussian_filter, then zoom(order=1, mode='mirror', grid_mode=True), then clip)
+// for the working-size outputs.
 //
 // The scipy stages accumulate in fp64 and round where scipy stores (fp32 arrays between passes, fp32 output of
 // map_coordinates on an fp32 input); additions and products are rounded one by one (__dadd_rn / __dmul_rn), as the
 // library's C code does them, so that no contraction changes the order of rounding.
+#include <limits.h>
 #include <math.h>
 
 #include "common.cuh"
@@ -187,14 +189,67 @@ __global__ void __launch_bounds__(kThreads) calib_ratio_kernel(const double* __r
   }
 }
 
+__device__ __forceinline__ float positive_nan_f() { return __int_as_float(0x7fc00000); }
+
+// ---- dense scale calibration (shutterstock/generate_frame_midas.py): ratio = nn / mvs where mvs > 1e-3 ---------------------
+// numpy's arithmetic for an fp32 MiDaS map nn and an MVS map of the stored dtype: for fp32 maps the threshold is 1e-3 rounded
+// to fp32 and the quotient is fp32; for fp64 maps nn is widened and the quotient is fp64. Elsewhere (NaN included) a positive
+// NaN, so that a device sort puts the rejected pixels last.
+__device__ __forceinline__ float dense_ratio(float nn, float m) { return m > 1e-3f ? __fdiv_rn(nn, m) : positive_nan_f(); }
+__device__ __forceinline__ double dense_ratio(float nn, double m) { return m > 1e-3 ? __ddiv_rn((double)nn, m) : positive_nan(); }
+
+__device__ __forceinline__ void load4(const float* p, float v[4]) {
+  const float4 a = __ldg(reinterpret_cast<const float4*>(p));
+  v[0] = a.x, v[1] = a.y, v[2] = a.z, v[3] = a.w;
+}
+__device__ __forceinline__ void load4(const double* p, double v[4]) {
+  const double2 a = __ldg(reinterpret_cast<const double2*>(p)), b = __ldg(reinterpret_cast<const double2*>(p) + 1);
+  v[0] = a.x, v[1] = a.y, v[2] = b.x, v[3] = b.y;
+}
+__device__ __forceinline__ void store4(float* p, const float v[4]) { *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]); }
+__device__ __forceinline__ void store4(double* p, const double v[4]) {
+  reinterpret_cast<double2*>(p)[0] = make_double2(v[0], v[1]);
+  reinterpret_cast<double2*>(p)[1] = make_double2(v[2], v[3]);
+}
+
+// one pass over the flat [N*HW] maps: groups of four elements with 16-byte loads when every base is 16-byte aligned, then the
+// remainder one element per thread
+template <typename M>
+__global__ void __launch_bounds__(kThreads) dense_ratio_kernel(const float* __restrict__ nn, const M* __restrict__ mvs,
+                                                                M* __restrict__ ratio, long n, int vec) {
+  DVD_PDL_ENTER();
+  const long tid = (long)blockIdx.x * blockDim.x + threadIdx.x, stride = (long)gridDim.x * blockDim.x;
+  long done = 0;
+  if (vec) {
+    const long nv = n / 4;
+    for (long i = tid; i < nv; i += stride) {
+      float a[4];
+      M b[4], r[4];
+      load4(nn + 4 * i, a);
+      load4(mvs + 4 * i, b);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) r[k] = dense_ratio(a[k], b[k]);
+      store4(ratio + 4 * i, r);
+    }
+    done = nv * 4;
+  }
+  for (long i = done + tid; i < n; i += stride) ratio[i] = dense_ratio(__ldg(nn + i), __ldg(mvs + i));
+}
+
 // np.median of each row's non-NaN entries, the row sorted ascending with NaN last: middle element, or the mean of the two
-// middle ones for an even count; count[f] = number of non-NaN entries (median NaN when 0). One thread per frame.
-__global__ void sorted_median_kernel(const double* __restrict__ sorted, double* __restrict__ med, int* __restrict__ count, int N,
-                                     long V) {
+// middle ones for an even count, (a + b) / 2 with the sum rounded to T as numpy's mean does; count[f] = number of non-NaN
+// entries (median NaN when 0). One thread per frame.
+__device__ __forceinline__ double mid_mean(double a, double b) { return __dadd_rn(a, b) / 2.0; }
+__device__ __forceinline__ float mid_mean(float a, float b) { return __fdiv_rn(__fadd_rn(a, b), 2.f); }
+__device__ __forceinline__ void set_nan(double* p) { *p = positive_nan(); }
+__device__ __forceinline__ void set_nan(float* p) { *p = positive_nan_f(); }
+
+template <typename T>
+__global__ void sorted_median_kernel(const T* __restrict__ sorted, T* __restrict__ med, int* __restrict__ count, int N, long V) {
   DVD_PDL_ENTER();
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= N) return;
-  const double* row = sorted + (long)f * V;
+  const T* row = sorted + (long)f * V;
   long lo = 0, hi = V;  // first NaN
   while (lo < hi) {
     const long mid = (lo + hi) / 2;
@@ -202,9 +257,9 @@ __global__ void sorted_median_kernel(const double* __restrict__ sorted, double* 
     else lo = mid + 1;
   }
   count[f] = (int)lo;
-  if (lo == 0) med[f] = positive_nan();
+  if (lo == 0) set_nan(med + f);
   else if (lo & 1) med[f] = row[lo / 2];
-  else med[f] = __dadd_rn(row[lo / 2 - 1], row[lo / 2]) / 2.0;
+  else med[f] = mid_mean(row[lo / 2 - 1], row[lo / 2]);
 }
 
 // ---- skimage.transform.resize(order=1, mode='reflect', anti_aliasing=True, preserve_range=True) on fp32 [N,H,W,C] ---------
@@ -377,7 +432,42 @@ extern "C" int dvd_sorted_median(const double* sorted, size_t sorted_bytes, int 
   FR_CHECK(aligned_to(sorted, 8) && aligned_to(median, 8) && aligned_to(count, 4), "dvd_sorted_median: misaligned buffer");
   FR_CHECK(sorted_bytes == (size_t)N * V * sizeof(double), "dvd_sorted_median: buffer %zu bytes, expected %zu", sorted_bytes,
            (size_t)N * V * sizeof(double));
-  DVD_CUDA_CALL(launch(sorted_median_kernel, dim3((N + 127) / 128), dim3(128), 0, (cudaStream_t)stream, sorted, median, count, N, V));
+  DVD_CUDA_CALL(launch(sorted_median_kernel<double>, dim3((N + 127) / 128), dim3(128), 0, (cudaStream_t)stream, sorted, median, count,
+                       N, V));
+  return 0;
+}
+
+extern "C" int dvd_sorted_median_f32(const float* sorted, size_t sorted_bytes, int N, long V, float* median, int* count,
+                                     void* stream) {
+  FR_CHECK(sorted && median && count, "dvd_sorted_median_f32: null pointer");
+  FR_CHECK(N >= 1 && V >= 1, "dvd_sorted_median_f32: bad shape N=%d V=%ld", N, V);
+  FR_CHECK(V <= INT_MAX, "dvd_sorted_median_f32: rows of %ld entries overflow the int32 count", V);
+  FR_CHECK(aligned_to(sorted, 4) && aligned_to(median, 4) && aligned_to(count, 4), "dvd_sorted_median_f32: misaligned buffer");
+  FR_CHECK(sorted_bytes == (size_t)N * V * sizeof(float), "dvd_sorted_median_f32: buffer %zu bytes, expected %zu", sorted_bytes,
+           (size_t)N * V * sizeof(float));
+  DVD_CUDA_CALL(launch(sorted_median_kernel<float>, dim3((N + 127) / 128), dim3(128), 0, (cudaStream_t)stream, sorted, median, count,
+                       N, V));
+  return 0;
+}
+
+extern "C" int dvd_dense_ratios(const float* nn, size_t nn_bytes, const void* mvs, size_t mvs_bytes, int mvs_f64, void* ratio,
+                                size_t ratio_bytes, int N, long HW, void* stream) {
+  FR_CHECK(nn && mvs && ratio, "dvd_dense_ratios: null pointer");
+  FR_CHECK(N >= 1 && HW >= 1 && (mvs_f64 == 0 || mvs_f64 == 1), "dvd_dense_ratios: bad arguments N=%d HW=%ld mvs_f64=%d", N, HW,
+           mvs_f64);
+  const size_t m = (size_t)N * HW, esz = mvs_f64 ? sizeof(double) : sizeof(float);
+  FR_CHECK(aligned_to(nn, 4) && aligned_to(mvs, esz) && aligned_to(ratio, esz), "dvd_dense_ratios: misaligned buffer");
+  FR_CHECK(nn_bytes == m * sizeof(float) && mvs_bytes == m * esz && ratio_bytes == m * esz,
+           "dvd_dense_ratios: buffer sizes %zu / %zu / %zu bytes, expected %zu / %zu / %zu", nn_bytes, mvs_bytes, ratio_bytes,
+           m * sizeof(float), m * esz, m * esz);
+  const int vec = aligned_to(nn, 16) && aligned_to(mvs, 16) && aligned_to(ratio, 16);
+  const long n = (long)m;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int grid = grid_for(vec ? (n + 3) / 4 : n);
+  if (mvs_f64)
+    DVD_CUDA_CALL(launch(dense_ratio_kernel<double>, dim3(grid), dim3(kThreads), 0, st, nn, (const double*)mvs, (double*)ratio, n, vec));
+  else
+    DVD_CUDA_CALL(launch(dense_ratio_kernel<float>, dim3(grid), dim3(kThreads), 0, st, nn, (const float*)mvs, (float*)ratio, n, vec));
   return 0;
 }
 

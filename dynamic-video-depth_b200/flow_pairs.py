@@ -4,7 +4,8 @@ The reference prepares a video in three steps: `generate_flows.py` resizes each 
 consistency masks on the CPU one pair at a time, `generate_sequence_midas.py` writes one `.pt` file per pair (2 MB each at
 384x224), and `datasets/davis_sequence.py` `torch.load`s one of them per step. `PairBuilder` does the same work once:
 
-  input   <frames>/frame_%05d.npz       img [H,W,3], pose_c2w, intrinsics, depth_mvs, depth_pred, optional motion_seg
+  input   <frames>/frame_%05d.npz       img [H,W,3], pose_c2w, intrinsics, depth_mvs, depth_pred, optional motion_seg (absent
+                                        or None: motion_seg_1 is then mask_2, as the ShutterStock generate_sequence_midas.py does)
           <flows>/flowpair_%05d_%05d.npz flow_1_2, flow_2_1 [h,w,2] and, when generate_flows.py wrote it, mask_1 / mask_2
   flows   a file that holds masks and flows at the frames' resolution is used as it is (it is exactly the reference's
           output); any other file is treated as raw flows at any resolution: all such pairs of one gap go through
@@ -34,8 +35,11 @@ def pair_list(n_frames, gaps):
 
 
 def read_npz(path):
+    """The arrays of an .npz file. An entry stored as None (a 0-d object array: the ShutterStock frame files write
+    motion_seg=None) is left out, so it reads as absent."""
     with np.load(path, allow_pickle=True) as d:
-        return {k: d[k] for k in d.keys()}
+        out = {k: d[k] for k in d.keys()}
+    return {k: v for k, v in out.items() if not (v.dtype == object and v.shape == () and v.item() is None)}
 
 
 def pose_tensors(im1, im2):

@@ -743,16 +743,47 @@ def calib_ratios(depth_coef, mask_coef, w2c, points, fx, fy, cx, cy, out=None):
 
 
 def row_medians(ratio):
-    """np.median of the non-NaN entries of each row of [N,V] fp64 -> (median [N] fp64, count [N] int32). The rows are sorted on
-    the device first (NaN last)."""
-    _chk_dtype(ratio, 'ratio', torch.float64, 2)
+    """np.median of the non-NaN entries of each row of [N,V] fp64 or fp32 -> (median [N] of the same dtype, count [N] int32).
+    The rows are sorted on the device first (NaN last). For fp32 rows the median is numpy's fp32 one: the middle element, or
+    the fp32 (a + b) / 2 of the two middle ones."""
+    if isinstance(ratio, torch.Tensor) and ratio.dtype == torch.float32:
+        _chk_dtype(ratio, 'ratio', torch.float32, 2)
+    else:
+        _chk_dtype(ratio, 'ratio', torch.float64, 2)
     N, V = ratio.shape
+    if V < 1 or V > 2 ** 31 - 1:
+        raise ValueError('ratio rows must hold 1 .. 2^31 - 1 entries, got %d' % V)
     srt = torch.sort(ratio, dim=1)[0].contiguous()
-    med = torch.empty(N, dtype=torch.float64, device=ratio.device)
+    med = torch.empty(N, dtype=ratio.dtype, device=ratio.device)
     cnt = torch.empty(N, dtype=torch.int32, device=ratio.device)
     LAUNCHES['n'] += 1
-    _lib.check(_lib.load().dvd_sorted_median(_ptr(srt), srt.numel() * 8, N, V, _ptr(med), _ptr(cnt), _stream()), 'dvd_sorted_median')
+    if ratio.dtype == torch.float32:
+        _lib.check(_lib.load().dvd_sorted_median_f32(_ptr(srt), srt.numel() * 4, N, V, _ptr(med), _ptr(cnt), _stream()),
+                   'dvd_sorted_median_f32')
+    else:
+        _lib.check(_lib.load().dvd_sorted_median(_ptr(srt), srt.numel() * 8, N, V, _ptr(med), _ptr(cnt), _stream()),
+                   'dvd_sorted_median')
     return med, cnt
+
+
+def dense_ratios(nn, mvs):
+    """The ShutterStock calibration's ratios (shutterstock/generate_frame_midas.py:167-172): nn [N,H,W] fp32 (MiDaS depth at the
+    stored size) and mvs [N,H,W] fp32 or fp64 -> [N,H*W] of mvs's dtype, nn / mvs where mvs > 1e-3 and a positive NaN
+    elsewhere, in numpy's arithmetic (fp32 threshold and quotient for fp32 maps). row_medians of the result gives the
+    per-frame medians of the script."""
+    _chk_dtype(nn, 'nn', torch.float32, 3)
+    if not isinstance(mvs, torch.Tensor) or mvs.dtype not in (torch.float32, torch.float64):
+        raise ValueError('mvs must be a float32 or float64 tensor, got %s' % getattr(mvs, 'dtype', type(mvs)))
+    _chk_dtype(mvs, 'mvs', mvs.dtype, 3)
+    if mvs.shape != nn.shape or mvs.device != nn.device or nn.numel() == 0:
+        raise ValueError('nn %s and mvs %s must be non-empty, of one shape, on one device' % (tuple(nn.shape), tuple(mvs.shape)))
+    N, H, W = nn.shape
+    out = torch.empty(N, H * W, dtype=mvs.dtype, device=nn.device)
+    es = mvs.element_size()
+    LAUNCHES['n'] += 1
+    _lib.check(_lib.load().dvd_dense_ratios(_ptr(nn), nn.numel() * 4, _ptr(mvs), mvs.numel() * es, int(es == 8), _ptr(out),
+                                            out.numel() * es, N, H * W, _stream()), 'dvd_dense_ratios')
+    return out
 
 
 def gaussian_weights(n_in, n_out):

@@ -342,7 +342,7 @@ int dvd_disp_vali_partials_size(int N, int H, int W);
 int dvd_disp_vali(const float* depth, const float* depth_gt, float* frame_sse, float* terms, float* partials, int N, int H, int W,
                   void* stream);
 
-/* ---- frame preparation (csrc/frame_prep.cu): scripts/preprocess/davis/generate_frame_midas.py ---------------------------------
+/* ---- frame preparation (csrc/frame_prep.cu): scripts/preprocess/{davis,shutterstock}/generate_frame_midas.py -------------------
  * Buffers are caller-allocated; byte sizes, shapes and alignment are checked before any launch (-2 with a message); nothing
  * synchronises. The scipy stages accumulate in fp64 and round to fp32 where scipy stores fp32.                                */
 /* F.interpolate(x, (H, W), mode='bicubic', align_corners=True) of NC planes: src [NC,h,w] -> dst [NC,H,W] fp32, any sizes (ATen's
@@ -365,6 +365,16 @@ int dvd_calib_ratios(const double* depth_coef, const double* mask_coef, size_t c
 /* np.median of the non-NaN entries of each row of sorted [N,V] (rows ascending, NaN last): median [N] fp64, count [N] int32
  * (the number of non-NaN entries; the median is NaN where it is 0).                                                           */
 int dvd_sorted_median(const double* sorted, size_t sorted_bytes, int N, long V, double* median, int* count, void* stream);
+/* The same for fp32 rows, with numpy's fp32 rule: the middle element, or the fp32 (a + b) / 2 of the two middle ones (the sum
+ * rounded to fp32). V <= INT_MAX.                                                                                              */
+int dvd_sorted_median_f32(const float* sorted, size_t sorted_bytes, int N, long V, float* median, int* count, void* stream);
+/* ShutterStock's dense calibration ratios (shutterstock/generate_frame_midas.py): nn [N,HW] fp32 (MiDaS depth at the stored
+ * size), mvs [N,HW] fp32 (mvs_f64 = 0) or fp64 (mvs_f64 = 1) -> ratio [N,HW] of mvs's dtype, ratio = nn / mvs where mvs > 1e-3
+ * and a positive NaN elsewhere (so that an ascending device sort puts the rejected pixels last). As numpy computes it: for
+ * fp32 maps the threshold is 1e-3 rounded to fp32 and the quotient is fp32; for fp64 maps, (double)nn / mvs. One pass, 16-byte
+ * loads when nn, mvs and ratio are 16-byte aligned.                                                                            */
+int dvd_dense_ratios(const float* nn, size_t nn_bytes, const void* mvs, size_t mvs_bytes, int mvs_f64, void* ratio,
+                     size_t ratio_bytes, int N, long HW, void* stream);
 /* skimage.transform.resize(src[n], (OH, OW), preserve_range=True) of fp32 [N,H,W,C] as skimage >= 0.19 computes it:
  * gaussian_filter along axis 0 with the weights wy [2 ry + 1], then axis 1 with wx [2 rx + 1] (fp64 device arrays; mode 'mirror',
  * each pass fp64 and stored fp32), zoom(order=1, mode='mirror', grid_mode=True) in fp64 rounded to fp32, then a clip to the
