@@ -46,9 +46,28 @@ Deliberate deviations from the ShutterStock script, all ValueError:
     most such sizes and otherwise predicts depth at a larger size than the image);
   * a working size of 0 (a side under 32 where the script rounds down);
   * a prediction/img that is not fp32 [H,W,3].
+
+COLMAP: ColmapFrameBuilder, the DAVIS computation on a COLMAP reconstruction of any posed video
+  input   a sparse model read by read_colmap_model (cameras, images, points3D as .bin, or as .txt when the .bin files are not
+          all there; one PINHOLE or SIMPLE_PINHOLE camera shared by every registered image), the registered images at
+          <images_dir>/<name>, and optionally masks at <masks_dir>/<name without its extension>.png (red channel, as DAVIS)
+  output  the DAVIS frame files, one per registered image in the sorted order of the names: the same keys, dtypes, working
+          size and intrinsics; motion_seg is all 0 without masks
+
+The model becomes what read_cameras returns for a DAVIS track, and FrameBuilder's device passes and frame() run unchanged on
+it. COLMAP's world-to-camera [R | t], R = qvec2rotmat(q), is already in the projection's camera axes (x right, y down, z
+forward), so no axis flip is applied. Deliberate deviations from what a DAVIS track of the same scene would hold:
+  * COLMAP puts the centre of the top-left pixel at (0.5, 0.5), the reference's projection and spline sampling at (0, 0):
+    the intrinsics carry cx - 0.5 and cy - 0.5;
+  * every point of points3D, in the order of the ids, goes to the calibration, as every .obj vertex does; the visibility
+    tracks are not used, so the in-image, mask and depth tests alone select the points;
+  * an image file in images_dir that the model did not register raises ValueError: dropping it would shift the time stamps
+    (idx / n_frames) of every later frame. So do a camera model other than PINHOLE or SIMPLE_PINHOLE, more than one camera,
+    a decoded image whose size is not the camera's, and a model without points or registered images.
 """
 import glob
 import os
+import struct
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
@@ -121,6 +140,13 @@ def frame_pose(w2c, s):
     return np.linalg.inv(T).astype(np.float32)
 
 
+def _net_device(net):
+    dev = next(net.parameters()).device
+    if dev.type != 'cuda' or net.training:
+        raise ValueError('midas_net must live on a CUDA device, in eval mode')
+    return dev
+
+
 def decode_image(path):
     return np.asarray(Image.open(path)).astype(np.float32) / 255
 
@@ -156,12 +182,11 @@ class FrameBuilder(_FrameFiles):
             raise ValueError('%d cameras for %d frames' % (self.extrinsics.shape[0], len(self.frames)))
         self.n_frames = len(self.frames)
         self.workers = workers
-        dev = next(midas_net.parameters()).device
-        if dev.type != 'cuda' or midas_net.training:
-            raise ValueError('midas_net must live on a CUDA device, in eval mode')
-        self._run(midas_net, h_pt, chunk, dev)
+        self._run(midas_net, h_pt, chunk, _net_device(midas_net))
 
     def _run(self, net, h_pt, chunk, dev):
+        """The device passes over self.frames and self.masks (mask paths, or None for all-zero masks) with the cameras
+        self.intrinsics, self.extrinsics and the points h_pt [4,V]."""
         N = self.n_frames
         points = torch.from_numpy(np.ascontiguousarray(h_pt[:3].T)).to(dev)
         w2c = torch.from_numpy(np.ascontiguousarray(self.extrinsics[:N])).to(dev)
@@ -174,8 +199,11 @@ class FrameBuilder(_FrameFiles):
             for a in range(0, N, chunk):
                 b = min(a + chunk, N)
                 imgs = np.stack(list(pool.map(decode_image, self.frames[a:b])))
-                masks = np.stack(list(pool.map(decode_mask, self.masks[a:b])))
                 n, H, W, _ = imgs.shape
+                if self.masks is None:                                             # every point passes the mask test
+                    masks = np.zeros((n, H, W), np.float32)
+                else:
+                    masks = np.stack(list(pool.map(decode_mask, self.masks[a:b])))
                 if a == 0:
                     self.size = (H, W)
                     self.target = working_size(H, W)
@@ -214,6 +242,245 @@ class FrameBuilder(_FrameFiles):
         return dict(img=img, pose_c2w=frame_pose(self.extrinsics[i], self.scale), depth_mvs=depth,
                     intrinsics=frame_intrinsics(self.intrinsics, H, W, th, tw), depth_pred=depth,
                     img_orig=decode_image(self.frames[i]), motion_seg=np.where(mask > 1e-3, 1, 0))
+
+
+# ---- COLMAP -------------------------------------------------------------------------------------------------------------------
+# model id -> (name, parameter count), as COLMAP's read_write_model.py lists them; the count is what skips a camera's record
+COLMAP_CAMERA_MODELS = {0: ('SIMPLE_PINHOLE', 3), 1: ('PINHOLE', 4), 2: ('SIMPLE_RADIAL', 4), 3: ('RADIAL', 5), 4: ('OPENCV', 8),
+                        5: ('OPENCV_FISHEYE', 8), 6: ('FULL_OPENCV', 12), 7: ('FOV', 5), 8: ('SIMPLE_RADIAL_FISHEYE', 4),
+                        9: ('RADIAL_FISHEYE', 5), 10: ('THIN_PRISM_FISHEYE', 12)}
+IMAGE_EXTS = ('.jpg', '.jpeg', '.png')
+
+
+def qvec2rotmat(q):
+    """COLMAP's rotation of a stored quaternion (w, x, y, z), [..., 4] -> [..., 3, 3] fp64, with its expressions as written
+    (the quaternion is not normalised)."""
+    q = np.asarray(q, dtype=np.float64)
+    w, x, y, z = q[..., 0], q[..., 1], q[..., 2], q[..., 3]
+    R = [[1 - 2 * y ** 2 - 2 * z ** 2, 2 * x * y - 2 * w * z, 2 * z * x + 2 * w * y],
+         [2 * x * y + 2 * w * z, 1 - 2 * x ** 2 - 2 * z ** 2, 2 * y * z - 2 * w * x],
+         [2 * z * x - 2 * w * y, 2 * y * z + 2 * w * x, 1 - 2 * x ** 2 - 2 * y ** 2]]
+    return np.stack([np.stack(r, -1) for r in R], -2)
+
+
+class _Reader:
+    """Little-endian fields of a COLMAP .bin file, read in order."""
+
+    def __init__(self, path):
+        self.path = path
+        with open(path, 'rb') as f:
+            self.data = f.read()
+        self.pos = 0
+
+    def read(self, fmt):
+        try:
+            v = struct.unpack_from('<' + fmt, self.data, self.pos)
+        except struct.error:
+            raise ValueError('%s ends inside a record' % self.path) from None
+        self.pos += struct.calcsize('<' + fmt)
+        return v
+
+    def name(self):
+        end = self.data.find(b'\0', self.pos)
+        if end < 0:
+            raise ValueError('%s ends inside an image name' % self.path)
+        s = self.data[self.pos:end].decode('utf-8')
+        self.pos = end + 1
+        return s
+
+    def done(self):
+        if self.pos > len(self.data):
+            raise ValueError('%s ends inside a record' % self.path)
+        if self.pos < len(self.data):
+            raise ValueError('%s has %d bytes after its last record' % (self.path, len(self.data) - self.pos))
+
+
+def _text_lines(path):
+    with open(path) as f:
+        return [ln.rstrip('\r\n') for ln in f]
+
+
+def _cameras_bin(path):
+    r = _Reader(path)
+    cams = {}
+    for _ in range(r.read('Q')[0]):
+        cid, model, w, h = r.read('iiQQ')
+        if model not in COLMAP_CAMERA_MODELS:
+            raise ValueError('%s: camera %d has the unknown model id %d, whose parameters cannot be skipped' % (path, cid, model))
+        name, k = COLMAP_CAMERA_MODELS[model]
+        cams[cid] = (name, w, h, r.read('%dd' % k))
+    r.done()
+    return cams
+
+
+def _cameras_txt(path):
+    cams = {}
+    for ln in _text_lines(path):
+        e = ln.split()
+        if e and not e[0].startswith('#'):
+            cams[int(e[0])] = (e[1], int(e[2]), int(e[3]), tuple(float(v) for v in e[4:]))
+    return cams
+
+
+def _images_bin(path):
+    """-> {image id: (qvec, tvec, camera id, name)}"""
+    r = _Reader(path)
+    imgs = {}
+    for _ in range(r.read('Q')[0]):
+        iid, *qt, cid = r.read('i7di')
+        name = r.name()
+        n2d = r.read('Q')[0]
+        r.pos += 24 * n2d                                    # (x, y, point3D id) per 2-D point: not used
+        imgs[iid] = (qt[:4], qt[4:], cid, name)
+    r.done()
+    return imgs
+
+
+def _images_txt(path):
+    imgs = {}
+    lines = iter(_text_lines(path))
+    for ln in lines:
+        if not ln.strip() or ln.lstrip().startswith('#'):
+            continue
+        e = ln.split(None, 9)
+        if len(e) < 10:
+            raise ValueError('%s: image line %r has no name' % (path, ln))
+        imgs[int(e[0])] = (tuple(float(v) for v in e[1:5]), tuple(float(v) for v in e[5:8]), int(e[8]), e[9].strip())
+        next(lines, None)                                    # its 2-D points, possibly an empty line
+    return imgs
+
+
+def _points_bin(path):
+    """-> (ids [V] uint64, xyz [V,3] fp64). A record is 51 bytes (u64 id, 3 f64, 3 u8, f64 error, u64 track length) followed
+    by 8 bytes (i32 image id, i32 point2D index) per track element, which are skipped."""
+    r = _Reader(path)
+    n = r.read('Q')[0]
+    data, pos, unpack = r.data, r.pos, struct.Struct('<Q3d3BdQ').unpack_from
+    ids, xyz = [], []
+    try:
+        for _ in range(n):
+            rec = unpack(data, pos)
+            ids.append(rec[0])
+            xyz.append(rec[1:4])
+            pos += 51 + 8 * rec[8]
+    except struct.error:
+        raise ValueError('%s ends inside a record' % path) from None
+    r.pos = pos
+    r.done()
+    return np.asarray(ids, np.uint64), np.asarray(xyz, np.float64).reshape(-1, 3)
+
+
+def _points_txt(path):
+    ids, xyz = [], []
+    for ln in _text_lines(path):
+        e = ln.split(None, 4)
+        if e and not e[0].startswith('#'):
+            ids.append(int(e[0]))
+            xyz.append([float(v) for v in e[1:4]])
+    return np.asarray(ids, np.uint64), np.asarray(xyz, np.float64).reshape(-1, 3)
+
+
+def _colmap_model(model_dir):
+    """read_colmap_model's values, and the camera's (height, width)."""
+    parts = ('cameras', 'images', 'points3D')
+    if all(os.path.isfile(os.path.join(model_dir, p + '.bin')) for p in parts):
+        readers, ext = (_cameras_bin, _images_bin, _points_bin), '.bin'
+    elif all(os.path.isfile(os.path.join(model_dir, p + '.txt')) for p in parts):
+        readers, ext = (_cameras_txt, _images_txt, _points_txt), '.txt'
+    else:
+        raise FileNotFoundError('%s holds neither cameras, images and points3D .bin nor the three .txt files' % model_dir)
+    cams, imgs, (ids, xyz) = (read(os.path.join(model_dir, p + ext)) for read, p in zip(readers, parts))
+    if not imgs:
+        raise ValueError('the model in %s has no registered image' % model_dir)
+    if not len(ids):
+        raise ValueError('the model in %s has no 3-D point' % model_dir)
+    used = sorted({im[2] for im in imgs.values()})
+    if len(used) != 1:
+        raise ValueError('the registered images use %d cameras (%s); the frame files need one camera for the whole video'
+                         % (len(used), used))
+    if used[0] not in cams:
+        raise ValueError('the registered images use camera %d, which the model does not hold' % used[0])
+    model, w, h, params = cams[used[0]]
+    if model == 'PINHOLE' and len(params) == 4:
+        fx, fy, cx, cy = params
+    elif model == 'SIMPLE_PINHOLE' and len(params) == 3:
+        fx, cx, cy = params
+        fy = fx
+    else:
+        raise ValueError('camera %d is %s with %d parameters; only PINHOLE and SIMPLE_PINHOLE are supported: undistort first: '
+                         '`colmap image_undistorter`' % (used[0], model, len(params)))
+    order = sorted(imgs.values(), key=lambda im: im[3])
+    names = [im[3] for im in order]
+    extrinsics = np.zeros([len(order), 4, 4])
+    extrinsics[:, :3, :3] = qvec2rotmat([im[0] for im in order])
+    extrinsics[:, :3, 3] = [im[1] for im in order]
+    extrinsics[:, 3, 3] = 1
+    h_pt = np.ones([len(ids), 4])
+    h_pt[:, :3] = xyz[np.argsort(ids, kind='stable')]
+    intrinsics = np.zeros([3, 3])
+    intrinsics[[0, 0, 1, 1, 2], [0, 2, 1, 2, 2]] = [fx, cx - 0.5, fy, cy - 0.5, 1]       # pixel centres at integers
+    return intrinsics, names, extrinsics, h_pt.T, (int(h), int(w))
+
+
+def read_colmap_model(model_dir):
+    """A COLMAP sparse model (cameras, images and points3D as .bin, or as .txt when the three .bin files are not all present)
+    -> (intrinsics [3,3] fp64 with cx - 0.5 and cy - 0.5, the registered image names sorted, extrinsics [N,4,4] fp64
+    world-to-camera [[qvec2rotmat(q), t], [0, 1]] in the order of the names, h_pt [4,V] fp64 of every point in the order of
+    the ids): what read_cameras returns for a DAVIS track. ValueError when the registered images do not share one PINHOLE or
+    SIMPLE_PINHOLE camera, or the model has no registered image or no point."""
+    return _colmap_model(model_dir)[:4]
+
+
+def colmap_frame_paths(images_dir, names, size):
+    """<images_dir>/<name> of each registered image. ValueError for an image file (.jpg, .jpeg, .png) under images_dir that is
+    not registered, or a registered image whose size is not size = (height, width); FileNotFoundError for a missing one."""
+    registered = set(names)
+    extra = []
+    for d, _, files in os.walk(images_dir):
+        for f in files:
+            rel = os.path.relpath(os.path.join(d, f), images_dir).replace(os.sep, '/')
+            if os.path.splitext(f)[1].lower() in IMAGE_EXTS and rel not in registered:
+                extra.append(rel)
+    if extra:
+        raise ValueError('%d image(s) under %s are not registered in the model; dropping them would shift the time of every '
+                         'later frame, so remove them or register them: %s' % (len(extra), images_dir, sorted(extra)))
+    paths = [os.path.join(images_dir, n) for n in names]
+    missing = [n for n, p in zip(names, paths) if not os.path.isfile(p)]
+    if missing:
+        raise FileNotFoundError('registered image(s) missing under %s: %s' % (images_dir, missing))
+    for n, p in zip(names, paths):
+        with Image.open(p) as im:
+            if (im.height, im.width) != tuple(size):
+                raise ValueError('image %s is %dx%d, its camera %dx%d (height x width)' % ((n, im.height, im.width) + tuple(size)))
+    return paths
+
+
+class ColmapFrameBuilder(FrameBuilder):
+    """Prepares the frames of a COLMAP reconstruction: the images registered in the sparse model under `model_dir`
+    (read_colmap_model), sorted by name, read from `images_dir`, with masks `<masks_dir>/<name without extension>.png` or, when
+    `masks_dir` is None, all-zero masks. FrameBuilder's device passes and outputs, on `midas_net` (a MidasNet on CUDA, eval
+    mode), `chunk` frames per pass. After construction: `names`, `scale` (s), `medians` [N], `counts` [N], `n_frames`, and
+    `frame(i)` / `write(out_dir)`.
+
+    Device memory: the ratios of every point in every frame, [N, V] fp64 (8·N·V bytes: 0.8 GB at N = 200, V = 5·10^5), stay
+    on the device until the per-frame medians, whose sort of all N rows at once takes about five times as much again (4.0 GB
+    at N = 200, V = 5·10^5, tools/bench_prepare_colmap.py); beside them, one chunk's full-resolution images and maps and the
+    working-size outputs of every frame. The points are never subsampled: that would change the medians."""
+
+    def __init__(self, images_dir, model_dir, midas_net, masks_dir=None, chunk=8, workers=8):
+        if chunk < 1:
+            raise ValueError('chunk must be >= 1, got %d' % chunk)
+        self.intrinsics, self.names, self.extrinsics, h_pt, size = _colmap_model(model_dir)
+        self.frames = colmap_frame_paths(images_dir, self.names, size)
+        self.masks = None
+        if masks_dir is not None:
+            self.masks = [os.path.join(masks_dir, os.path.splitext(n)[0] + '.png') for n in self.names]
+            missing = [p for p in self.masks if not os.path.isfile(p)]
+            if missing:
+                raise FileNotFoundError('%d mask(s) missing: %s' % (len(missing), missing))
+        self.n_frames = len(self.frames)
+        self.workers = workers
+        self._run(midas_net, h_pt, chunk, _net_device(midas_net))
 
 
 # ---- ShutterStock -------------------------------------------------------------------------------------------------------------
