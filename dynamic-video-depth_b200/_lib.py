@@ -132,13 +132,19 @@ SIGNATURES = {
     'dvd_dense_ratios': [_P, ctypes.c_size_t, _P, ctypes.c_size_t, _I, _P, ctypes.c_size_t, _I, ctypes.c_long, _P],
     'dvd_aa_resize_scratch_bytes': [_I, _I, _I, _I],
     'dvd_aa_resize': [_P, ctypes.c_size_t, _P, ctypes.c_size_t, _P, ctypes.c_size_t, _P, _I, _P, _I, _I, _I, _I, _I, _I, _I, _P],
+    'dvd_points_select_scratch_bytes': [_I, _I, _I],
+    'dvd_points_select': [_P, _P, _P, _I, _I, _I, ctypes.c_double, ctypes.c_double, _L, _L, _L, _L, _P, _P, _P, _P, _P, _P,
+                          ctypes.c_size_t, ctypes.POINTER(_L), _P],
+    'dvd_voxel_reduce_scratch_bytes': [_L],
+    'dvd_voxel_reduce': [_P, _P, _P, _P, _P, _L, _L, _I, _P, _P, _P, _P, _P, ctypes.c_size_t, ctypes.POINTER(_L), _P],
 }
 DVD_MASKS_FLOWPAIR_U8 = 0
 DVD_MASKS_PAIRFILE_F32 = 1
 _RESTYPES = {'dvd_last_error': ctypes.c_char_p, 'dvd_struct_size': ctypes.c_long, 'dvd_conv2d_workspace_bytes': ctypes.c_size_t, 'dvd_conv2d_pack_blocks': ctypes.c_long, 'dvd_mlp_packed_weights_bytes': ctypes.c_size_t,
              'dvd_mlp_save_bytes_per_eval': ctypes.c_size_t, 'dvd_mlp_dy_bytes': ctypes.c_size_t,
              'dvd_raft_instnorm_scratch_bytes': ctypes.c_long, 'dvd_raft_pyramid_floats': ctypes.c_long,
-             'dvd_aa_resize_scratch_bytes': ctypes.c_long}
+             'dvd_aa_resize_scratch_bytes': ctypes.c_long, 'dvd_points_select_scratch_bytes': ctypes.c_long,
+             'dvd_voxel_reduce_scratch_bytes': ctypes.c_long}
 
 _lib = None
 

@@ -825,3 +825,75 @@ def aa_resize(src, OH, OW, weights=None):
     _lib.check(lib.dvd_aa_resize(_ptr(src), src.numel() * 4, _ptr(out), out.numel() * 4, _ptr(scratch), nb, _ptr(wy),
                                  wy.numel() // 2, _ptr(wx), wx.numel() // 2, N, H, W, C, OH, OW, _stream()), 'dvd_aa_resize')
     return out
+
+
+# ---- point-cloud export (csrc/points.cu) -------------------------------------------------------------------------------------
+class KeyRangeError(ValueError):
+    """A voxel key left the 2^21-voxel range of an axis."""
+
+
+def points_select(depth, img, P, edge_tol, voxel=None, origin=(0, 0, 0), base=0):
+    """dvd_points_select: depth [N,H,W], img [N,3,H,W], P [N,3,H,W] fp32 -> dict of the kept pixels in pixel order: mask [N,H,W]
+    uint8 (all pixels), index [M] int64 (base + flat pixel index), xyz [M,3] fp32, rgb [M,3] uint8 and, with a voxel size,
+    key [M] int64 relative to the voxel `origin`. Waits for the stream (M sizes the outputs). Raises KeyRangeError when a key
+    is out of range."""
+    _chk(depth, 'depth')
+    if depth.dim() != 3:
+        raise ValueError('depth must be [N,H,W], got %s' % (tuple(depth.shape),))
+    N, H, W = depth.shape
+    _chk(img, 'img', (N, 3, H, W)), _chk(P, 'P', (N, 3, H, W))
+    if img.device != depth.device or P.device != depth.device:
+        raise ValueError('depth, img and P must be on one device')
+    dev, n = depth.device, N * H * W
+    lib = _lib.load()
+    scratch = torch.empty(lib.dvd_points_select_scratch_bytes(N, H, W), dtype=torch.uint8, device=dev)
+    mask = torch.empty(N, H, W, dtype=torch.uint8, device=dev)
+    key = torch.empty(n, dtype=torch.int64, device=dev) if voxel is not None else None
+    index = torch.empty(n, dtype=torch.int64, device=dev)
+    xyz = torch.empty(n, 3, dtype=torch.float32, device=dev)
+    rgb = torch.empty(n, 3, dtype=torch.uint8, device=dev)
+    m = ctypes.c_longlong(0)
+    LAUNCHES['n'] += 3
+    ox, oy, oz = (int(o) for o in origin)
+    rc = lib.dvd_points_select(_ptr(depth), _ptr(img), _ptr(P), N, H, W, float(edge_tol), float(voxel or 0.0), ox, oy, oz, int(base),
+                               _ptr(mask), _ptr(key), _ptr(index), _ptr(xyz), _ptr(rgb), _ptr(scratch), scratch.numel(),
+                               ctypes.byref(m), _stream())
+    if rc == -3:
+        raise KeyRangeError(lib.dvd_last_error().decode())
+    _lib.check(rc, 'dvd_points_select')
+    M = m.value
+    out = {'mask': mask, 'index': index[:M], 'xyz': xyz[:M], 'rgb': rgb[:M]}
+    if key is not None:
+        out['key'] = key[:M]
+    return out
+
+
+def voxel_reduce(skey, order, index, xyz, rgb, hw, min_views):
+    """dvd_voxel_reduce: skey [M] sorted int64 keys, order [M] int64 the stable sort's permutation of the items index [M] int64,
+    xyz [M,3] fp32, rgb [M,3] uint8 (frame = index // hw) -> dict of the runs seen in >= min_views frames, in key order: xyz,
+    rgb [R,3] fp64 means, count, views [R] int32. Waits for the stream (R sizes the outputs)."""
+    M = skey.numel()
+    for name, t, dt in (('skey', skey, torch.int64), ('order', order, torch.int64), ('index', index, torch.int64),
+                        ('xyz', xyz, torch.float32), ('rgb', rgb, torch.uint8)):
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != dt or not t.is_contiguous() or t.shape[0] != M:
+            raise ValueError('%s must be a contiguous CUDA %s tensor with %d rows' % (name, dt, M))
+    if tuple(xyz.shape) != (M, 3) or tuple(rgb.shape) != (M, 3):
+        raise ValueError('xyz and rgb must be [%d,3]' % M)
+    dev = skey.device
+    if M == 0:
+        z = torch.empty(0, 3, dtype=torch.float64, device=dev)
+        return {'xyz': z, 'rgb': z.clone(), 'count': torch.empty(0, dtype=torch.int32, device=dev),
+                'views': torch.empty(0, dtype=torch.int32, device=dev)}
+    lib = _lib.load()
+    scratch = torch.empty(lib.dvd_voxel_reduce_scratch_bytes(M), dtype=torch.uint8, device=dev)
+    mx = torch.empty(M, 3, dtype=torch.float64, device=dev)
+    mc = torch.empty(M, 3, dtype=torch.float64, device=dev)
+    cnt = torch.empty(M, dtype=torch.int32, device=dev)
+    views = torch.empty(M, dtype=torch.int32, device=dev)
+    r = ctypes.c_longlong(0)
+    LAUNCHES['n'] += 6
+    _lib.check(lib.dvd_voxel_reduce(_ptr(skey), _ptr(order), _ptr(index), _ptr(xyz), _ptr(rgb), M, int(hw), int(min_views), _ptr(mx),
+                                    _ptr(mc), _ptr(cnt), _ptr(views), _ptr(scratch), scratch.numel(), ctypes.byref(r), _stream()),
+               'dvd_voxel_reduce')
+    R = r.value
+    return {'xyz': mx[:R], 'rgb': mc[:R], 'count': cnt[:R], 'views': views[:R]}

@@ -383,6 +383,27 @@ long dvd_aa_resize_scratch_bytes(int N, int H, int W, int C);
 int dvd_aa_resize(const float* src, size_t src_bytes, float* dst, size_t dst_bytes, void* scratch, size_t scratch_bytes,
                   const double* wy, int ry, const double* wx, int rx, int N, int H, int W, int C, int OH, int OW, void* stream);
 
+/* ---- point-cloud export (csrc/points.cu). Both calls compact in index order with a tile count, a one-block scan of the tile
+ * counts and a scatter: no atomic decides a position, so equal inputs give bitwise equal outputs. Both wait for the stream and
+ * return the number of items written in *n_valid / *n_out. Scratch is 8-byte aligned, of the size the _scratch_bytes call gives. */
+/* depth [N,H,W], img [N,3,H,W], P [N,3,H,W] (dvd_unproject_fwd of the depth) fp32. Pixel i = (n H + y) W + x is kept when its
+ * depth d is finite and > 1e-2f and |d - d_n| / d <= edge_tol in fp64 for every in-image 4-neighbour n (NaN fails). mask [N H W]
+ * = 0 / 1. For the k-th kept pixel in pixel order: index[k] = base + i, xyz[k,3] = P, rgb[k,3] = (uint8)(255 * clip(img, 0, 1))
+ * in fp32 (NaN -> 0) and, when key is not NULL, key[k] = (kx << 42) | (ky << 21) | kz with k_a = floor((double)P_a / voxel) -
+ * o_a. A k_a outside [0, 2^21) stores key -1 and returns -3 after the outputs are written. Capacity of the outputs: N H W.      */
+long dvd_points_select_scratch_bytes(int N, int H, int W);
+int dvd_points_select(const float* depth, const float* img, const float* P, int N, int H, int W, double edge_tol, double voxel,
+                      long long ox, long long oy, long long oz, long long base, unsigned char* mask, long long* key, long long* index,
+                      float* xyz, unsigned char* rgb, void* scratch, size_t scratch_bytes, long long* n_valid, void* stream);
+/* skey [M] ascending, order [M] the permutation that sorted them (point j of a run is item order[j] of index / xyz / rgb, and
+ * the items of one key come in ascending index, as a stable sort leaves them). For each run of equal keys, in run order: the
+ * fp64 means of xyz and rgb summed in sorted order, the point count and views = the number of distinct frames index / hw. Runs
+ * with views < min_views are dropped. Capacity of the outputs: M runs (mean_xyz, mean_rgb [M,3] fp64, count, views [M] int32). */
+long dvd_voxel_reduce_scratch_bytes(long long M);
+int dvd_voxel_reduce(const long long* skey, const long long* order, const long long* index, const float* xyz, const unsigned char* rgb,
+                     long long M, long long hw, int min_views, double* mean_xyz, double* mean_rgb, int* count, int* views,
+                     void* scratch, size_t scratch_bytes, long long* n_out, void* stream);
+
 /* ---- RAFT optical flow, forward only (csrc/raft_ops.cu): third_party/RAFT/core as scripts/preprocess/davis/generate_flows.py runs it
  * (large model, all-pairs correlation, 4 levels, radius 4, hidden = context = 128, no warm start, test_mode). These are the CUDA-core
  * stages; the convolutions between them are dvd_conv2d_nhwc launches (dvd_b200/raft.py holds the schedule). All tensors NHWC fp32,
