@@ -52,6 +52,17 @@ class MlpCfg(ctypes.Structure):
                 ('freq_t', ctypes.c_float * DVD_MLP_MAX_FREQ_T)]
 
 
+class VisPanel(ctypes.Structure):
+    """struct dvd_vis_panel (include/dvd_b200.h)."""
+    _fields_ = [('src', ctypes.c_void_p), ('vmin', ctypes.c_void_p), ('vmax', ctypes.c_void_p), ('s_canvas', ctypes.c_longlong),
+                ('s_row', ctypes.c_longlong), ('s_col', ctypes.c_longlong), ('s_chan', ctypes.c_longlong), ('rows', ctypes.c_int),
+                ('cols', ctypes.c_int), ('y0', ctypes.c_int), ('x0', ctypes.c_int), ('transform', ctypes.c_int),
+                ('reserved', ctypes.c_int)]
+
+
+DVD_VIS_DISP, DVD_VIS_GT_DISP, DVD_VIS_RGB = 0, 1, 2
+DVD_VIS_MAX_PANELS = 4
+
 _I, _F, _P = ctypes.c_int, ctypes.c_float, ctypes.c_void_p
 _L = ctypes.c_longlong
 
@@ -137,6 +148,7 @@ SIGNATURES = {
                           ctypes.c_size_t, ctypes.POINTER(_L), _P],
     'dvd_voxel_reduce_scratch_bytes': [_L],
     'dvd_voxel_reduce': [_P, _P, _P, _P, _P, _L, _L, _I, _P, _P, _P, _P, _P, ctypes.c_size_t, ctypes.POINTER(_L), _P],
+    'dvd_vis_panels': [_P, _L, _I, _I, _I, ctypes.POINTER(VisPanel), _I, _P, _P, _P],
 }
 DVD_MASKS_FLOWPAIR_U8 = 0
 DVD_MASKS_PAIRFILE_F32 = 1

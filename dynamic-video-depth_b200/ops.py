@@ -897,3 +897,63 @@ def voxel_reduce(skey, order, index, xyz, rgb, hw, min_views):
                'dvd_voxel_reduce')
     R = r.value
     return {'xyz': mx[:R], 'rgb': mc[:R], 'count': cnt[:R], 'views': views[:R]}
+
+
+# ---- test-end visualisation (csrc/test_videos.cu) -----------------------------------------------------------------------------
+VIS_TRANSFORMS = {'disp': _lib.DVD_VIS_DISP, 'gt_disp': _lib.DVD_VIS_GT_DISP, 'rgb': _lib.DVD_VIS_RGB}
+
+
+def vis_panel(src, transform, rows, cols, y0, x0, strides, offset=0, vmin=None, vmax=None):
+    """One panel of `vis_panels`: pixel (y0 + y, x0 + x) of canvas c reads element offset + c·s_canvas + y·s_row + x·s_col
+    (+ k·s_chan for channel k of 'rgb') of the contiguous fp32 CUDA tensor `src`; strides = (s_canvas, s_row, s_col, s_chan) in
+    elements. 'disp' and 'gt_disp' are colour-mapped through vmin[c], vmax[c] (contiguous fp64 CUDA tensors)."""
+    if transform not in VIS_TRANSFORMS:
+        raise ValueError('transform must be one of %s, got %r' % (sorted(VIS_TRANSFORMS), transform))
+    return dict(src=src, transform=transform, rows=int(rows), cols=int(cols), y0=int(y0), x0=int(x0),
+                strides=tuple(int(s) for s in strides), offset=int(offset), vmin=vmin, vmax=vmax)
+
+
+def vis_panels(tmpl, panels, lut, out, tmpl_stride=0):
+    """dvd_vis_panels: writes out [n,CH,CW,3] uint8 (BGR): canvas c = the template tmpl[c·tmpl_stride bytes …] ([CH,CW,3] uint8;
+    tmpl_stride = 0 shares one template) with the pixels of each `vis_panel` replaced. lut: [256,3] uint8 BGR colour table.
+    Every read a panel makes is checked against its source tensor before the launch."""
+    _chk_dtype(out, 'out', torch.uint8, 4)
+    n, CH, CW, C = out.shape
+    if C != 3:
+        raise ValueError('out must be [n,CH,CW,3], got %s' % (tuple(out.shape),))
+    if not isinstance(tmpl, torch.Tensor) or not tmpl.is_cuda or tmpl.dtype != torch.uint8 or not tmpl.is_contiguous():
+        raise ValueError('tmpl must be a contiguous uint8 CUDA tensor')
+    tmpl_stride = int(tmpl_stride)
+    if tmpl_stride < 0 or tmpl.numel() < (n - 1) * tmpl_stride + CH * CW * 3:
+        raise ValueError('tmpl holds %d bytes, %d canvases of %dx%d at stride %d need more' % (tmpl.numel(), n, CH, CW, tmpl_stride))
+    if len(panels) > _lib.DVD_VIS_MAX_PANELS:
+        raise ValueError('at most %d panels per call, got %d' % (_lib.DVD_VIS_MAX_PANELS, len(panels)))
+    arr = (_lib.VisPanel * max(len(panels), 1))()
+    mapped = False
+    for q, p in enumerate(panels):
+        src = _chk(p['src'], 'panels[%d].src' % q)
+        if src.device != out.device or tmpl.device != out.device:
+            raise ValueError('panels[%d]: the sources, the template and out must be on one device' % q)
+        s = p['strides']
+        if len(s) != 4 or min(s) < 0 or p['offset'] < 0:
+            raise ValueError('panels[%d]: strides %s and offset %d must be 4 non-negative integers' % (q, s, p['offset']))
+        last = p['offset'] + (n - 1) * s[0] + (p['rows'] - 1) * s[1] + (p['cols'] - 1) * s[2] + (2 * s[3] if p['transform'] == 'rgb' else 0)
+        if p['rows'] < 1 or p['cols'] < 1 or last >= src.numel():
+            raise ValueError('panels[%d]: %dx%d panel reads element %d of a %d-element source' % (q, p['rows'], p['cols'], last, src.numel()))
+        rng = (0, 0)
+        if p['transform'] != 'rgb':
+            mapped = True
+            for name in ('vmin', 'vmax'):
+                t = p[name]
+                if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float64 or not t.is_contiguous() or t.numel() < n:
+                    raise ValueError('panels[%d].%s must be a contiguous fp64 CUDA tensor of at least %d values' % (q, name, n))
+            rng = (p['vmin'].data_ptr(), p['vmax'].data_ptr())
+        arr[q] = _lib.VisPanel(src.data_ptr() + 4 * p['offset'], rng[0], rng[1], *s, p['rows'], p['cols'], p['y0'], p['x0'],
+                               VIS_TRANSFORMS[p['transform']], 0)
+    if mapped and (not isinstance(lut, torch.Tensor) or not lut.is_cuda or lut.dtype != torch.uint8 or not lut.is_contiguous()
+                   or tuple(lut.shape) != (256, 3)):
+        raise ValueError('lut must be a contiguous [256,3] uint8 CUDA tensor')
+    LAUNCHES['n'] += 1
+    _lib.check(_lib.load().dvd_vis_panels(_ptr(tmpl), tmpl_stride, n, CH, CW, arr, len(panels), _ptr(lut if mapped else None),
+                                          _ptr(out), _stream()), 'dvd_vis_panels')
+    return out

@@ -5,9 +5,15 @@ scene_flow_motion_field --dataset <alias> --checkpoint_path <training log dir> -
 Loads the training options from <checkpoint_path>/opt.pt and the weights from best.pt (--epoch < 0) or nets/<epoch>.pt, reads
 the dataset's `vali` frames once and keeps them on the GPU, and writes one
 <output_dir><net>_<dataset>[_<suffix>]/epoch{best|%04d}_test/batch%04d.npz per batch with the refined depth, the scene flow and
-the reference's `pack_output` keys (Model.test_on_batch). The reference's `on_test_end` videos and HTML page are not produced.
+the reference's `pack_output` keys (Model.test_on_batch). With `--videos [--slice_rows a:b]` it then writes the comparison and
+RGB frames, the temporal slices, their videos and the HTML page of the reference's `on_test_end` (dvd_b200/test_videos.py).
+These two flags are this driver's own (the reference has no such switch): they are taken off the command line before the
+rest goes to options_test, so the reference's flag surface stays as it is.
 """
+import argparse
 import os
+import re
+import sys
 from argparse import Namespace
 from os.path import join
 from shutil import rmtree
@@ -18,6 +24,7 @@ from .datasets import get_dataset
 from .models import get_model
 from .models.netinterface import NullLogger
 from .options import options_test
+from .test_videos import render_test_videos
 
 
 def output_dir_for(opt):
@@ -34,7 +41,20 @@ def output_dir_for(opt):
     return out
 
 
+def parse_video_flags(argv=None):
+    """(--videos, --slice_rows, the remaining arguments) of a test command line."""
+    argv = sys.argv[1:] if argv is None else list(argv)
+    p = argparse.ArgumentParser(add_help=False, allow_abbrev=False)
+    p.add_argument('--videos', action='store_true')
+    p.add_argument('--slice_rows', default=None)
+    flags, rest = p.parse_known_args(argv)
+    if flags.slice_rows is not None and not re.fullmatch(r'\d+:\d+', flags.slice_rows):
+        p.error('--slice_rows must look like a:b, got %r' % flags.slice_rows)   # before the export, not after it
+    return flags.videos, flags.slice_rows, rest
+
+
 def main(argv=None):
+    videos, slice_rows, argv = parse_video_flags(argv)
     opt = options_test.parse(argv)
     if opt.gpu == '-1':
         raise SystemExit('dvd_b200 has no CPU path (--gpu -1 is the reference CPU mode; use the reference for that)')
@@ -61,7 +81,11 @@ def main(argv=None):
     model.opt.epoch = opt.epoch
     for i, batch in enumerate(batches):
         model.test_on_batch(i, batch)
-    print('wrote %d batches to %s' % (len(batches), join(output_dir, 'epoch%s_test' % ('best' if opt.epoch < 0 else '%04d' % opt.epoch))))
+    test_dir = join(output_dir, 'epoch%s_test' % ('best' if opt.epoch < 0 else '%04d' % opt.epoch))
+    print('wrote %d batches to %s' % (len(batches), test_dir))
+    if videos:
+        res = render_test_videos(test_dir, slice_rows)
+        print('wrote the test videos and %s' % res['html'])
 
 
 if __name__ == '__main__':

@@ -45,7 +45,8 @@ enum { DVD_S_FLOW = 0, DVD_S_DISP = 1, DVD_S_SF = 2, DVD_S_LOSS = 3, DVD_S_MASKS
 
 const char* dvd_last_error(void);
 int dvd_version(void);
-/* sizeof of the structs passed by pointer: 0 dvd_loss_cfg, 1 dvd_mlp_cfg, 2 dvd_conv_desc, 3 dvd_pack_item (-1 otherwise) */
+/* sizeof of the structs passed by pointer: 0 dvd_loss_cfg, 1 dvd_mlp_cfg, 2 dvd_conv_desc, 3 dvd_pack_item, 4 dvd_vis_panel
+ * (-1 otherwise) */
 long dvd_struct_size(int which);
 /* number of fp32 partial-sum slots dvd_reproject_loss_fwd needs in `partials` for a given shape */
 int dvd_reproject_partials_size(int B, int H, int W);
@@ -403,6 +404,32 @@ long dvd_voxel_reduce_scratch_bytes(long long M);
 int dvd_voxel_reduce(const long long* skey, const long long* order, const long long* index, const float* xyz, const unsigned char* rgb,
                      long long M, long long hw, int min_views, double* mean_xyz, double* mean_rgb, int* count, int* views,
                      void* scratch, size_t scratch_bytes, long long* n_out, void* stream);
+
+/* ---- test-end visualisation (csrc/test_videos.cu): models/video_base.py:157-272 (on_test_end) without matplotlib. ----------- */
+#define DVD_VIS_MAX_PANELS 4
+enum { DVD_VIS_DISP = 0, DVD_VIS_GT_DISP = 1, DVD_VIS_RGB = 2 };
+/* One panel of a canvas batch. Pixel (y0 + y, x0 + x) of canvas c reads src[c s_canvas + y s_row + x s_col (+ k s_chan for
+ * channel k of DVD_VIS_RGB)], strides in elements, so a temporal slice depth[:, 0, r, :] is read in place (s_canvas = W,
+ * s_row = H W, s_col = 1). Transforms: DVD_VIS_DISP v = 1 / x in fp32; DVD_VIS_GT_DISP v = [x > 1e-8f] / (double)(x + 1e-8f)
+ * in fp64; both colour-mapped through the range (vmin[c], vmax[c]) (device fp64, one entry per canvas). DVD_VIS_RGB writes
+ * floor(255 clip(x, 0, 1)) per channel (NaN -> 0) as B, G, R; vmin / vmax are unused and may be NULL.                         */
+typedef struct dvd_vis_panel {
+  const float* src;
+  const double* vmin;
+  const double* vmax;
+  long long s_canvas, s_row, s_col, s_chan;
+  int rows, cols;
+  int y0, x0;
+  int transform;
+  int reserved; /* 0 */
+} dvd_vis_panel;
+/* out [n_canvas, CH, CW, 3] uint8 BGR: canvas c is a copy of tmpl + c tmpl_stride ([CH, CW, 3] uint8, tmpl_stride = 0 shares one
+ * template) with each panel's pixels replaced. Colour mapping: t = (v - vmin) / (vmax - vmin) in fp64, index floor(256 t)
+ * clamped to [0, 255] (matplotlib's Colormap rule with N = 256; vmax == vmin -> 0), lut [256, 3] BGR; NaN v or t -> black.
+ * `panels` is a HOST array of n_panels <= DVD_VIS_MAX_PANELS panels that lie inside the canvas and do not overlap (-1 otherwise).
+ * One thread writes 8 consecutive pixels of a row; every output byte is written once, no atomics.                             */
+int dvd_vis_panels(const unsigned char* tmpl, long long tmpl_stride, int n_canvas, int CH, int CW, const dvd_vis_panel* panels,
+                   int n_panels, const unsigned char* lut, unsigned char* out, void* stream);
 
 /* ---- RAFT optical flow, forward only (csrc/raft_ops.cu): third_party/RAFT/core as scripts/preprocess/davis/generate_flows.py runs it
  * (large model, all-pairs correlation, 4 levels, radius 4, hidden = context = 128, no warm start, test_mode). These are the CUDA-core
