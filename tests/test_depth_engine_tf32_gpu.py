@@ -102,37 +102,35 @@ def _cotangent(kind, N, H, W):
     return (1e-3 * (1 + 0.5 * torch.sin(9.0 * yy + ph) * torch.cos(7.0 * xx - ph))).cuda()
 
 
-def _check_engine_against_emulation(N, H, W, kind):
-    from oracle.midas_tf32 import Anchors, anchor_names, engine_anchors, midas_tf32_forward
-    net = _net()
+def capture_engine(net):
+    """What the emulation is teacher-forced with, read after a training forward of `net` and before anything re-packs its weights:
+    the engine's saved tensors as anchors (plus the down-sample branch outputs, which the engine recomputes rather than saves)
+    and its packed weight images in weight layout."""
+    from oracle.midas_tf32 import engine_anchors
     eng = net.engine()
-    names = _conv_names(net)
-    x = torch.rand(N, 3, H, W, generator=torch.Generator().manual_seed(3)).cuda()
-    cot = _cotangent(kind, N, H, W)
-    for p in net.parameters():
-        p.grad = None
-    depth = eng.forward(x, train=True)
-    S = eng.saved
-    eng.backward(cot)
-    A = engine_anchors(S)
+    A = engine_anchors(eng.saved)
     bi = 0
     for st in eng.stages:
         for b in st:
             if b.ds is not None:
                 A['block%d.ds' % bi] = b.ds.fwd(A['block%d.cur' % bi], round_out=False)
             bi += 1
-    images = _images(eng, names)
-    torch.cuda.synchronize()
-    del S
+    return A, _images(eng, _conv_names(net))
 
-    sd = {k: (v.detach().double().clone().requires_grad_() if (v.dtype.is_floating_point and 'running' not in k) else v.double())
-          for k, v in net.state_dict().items()}
+
+def check_engine_against_emulation(sd, x, depth, cot, A, images, grads, tag):
+    """The emulation of the forward that produced `depth` from images `x` (state dict `sd`, anchors and images from
+    capture_engine), its backward from the cotangent `cot`, against the engine: every anchor and the depth map, then every
+    parameter gradient in `grads` (name -> the engine's .grad)."""
+    from oracle.midas_tf32 import Anchors, anchor_names, midas_tf32_forward
+    sd = {k: (v.detach().cuda().double().clone().requires_grad_() if (v.dtype.is_floating_point and 'running' not in k)
+              else v.cuda().double()) for k, v in sd.items()}
     anc = Anchors(A)
     torch.cuda.reset_peak_memory_stats()
     d_emu = midas_tf32_forward(sd, x.double(), images=images, anchors=anc)
     (d_emu * cot.double()).sum().backward()
     torch.cuda.synchronize()
-    print('\n[%dx%dx%d %s] emulation peak memory %.1f GB' % (N, H, W, kind, torch.cuda.max_memory_allocated() / 2 ** 30))
+    print('\n[%s] emulation peak memory %.1f GB' % (tag, torch.cuda.max_memory_allocated() / 2 ** 30))
 
     # ---- forward
     rep = anc.report
@@ -161,18 +159,34 @@ def _check_engine_against_emulation(N, H, W, kind):
 
     # ---- backward: every parameter tensor
     report = []
-    for k, p in net.named_parameters():
+    for k, g in grads.items():
         ref = sd[k].grad
         if ref is None:         # refinenet4.resConfUnit1 is not part of the net's graph
-            assert float(p.grad.abs().max()) == 0.0, k
+            assert float(g.abs().max()) == 0.0, k
             continue
-        report.append((k,) + grad_agreement(p.grad, ref))
-    assert len(report) == sum(1 for _ in net.parameters()) - 4
+        report.append((k,) + grad_agreement(g, ref))
+    assert len(report) == len(grads) - 4
     for i, what in ((1, '|slope - 1|'), (2, 'rel L2'), (3, 'max-norm')):
         top = sorted(report, key=lambda r: -abs(r[i]))[:3]
         print('backward %s: ' % what + ', '.join('%s %.2e' % (r[0], abs(r[i])) for r in top))
     bad = [r for r in report if abs(r[1]) > GRAD_SLOPE or r[2] > GRAD_L2 or r[3] > GRAD_MAX]
     assert not bad, bad
+    return report
+
+
+def _check_engine_against_emulation(N, H, W, kind):
+    net = _net()
+    eng = net.engine()
+    x = torch.rand(N, 3, H, W, generator=torch.Generator().manual_seed(3)).cuda()
+    cot = _cotangent(kind, N, H, W)
+    for p in net.parameters():
+        p.grad = None
+    depth = eng.forward(x, train=True)
+    A, images = capture_engine(net)
+    eng.backward(cot)
+    torch.cuda.synchronize()
+    check_engine_against_emulation(net.state_dict(), x, depth, cot, A, images,
+                                   {k: p.grad for k, p in net.named_parameters()}, '%dx%dx%d %s' % (N, H, W, kind))
 
 
 @pytest.mark.parametrize('kind', ['smooth', 'white'])
