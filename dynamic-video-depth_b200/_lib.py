@@ -63,6 +63,16 @@ class VisPanel(ctypes.Structure):
 DVD_VIS_DISP, DVD_VIS_GT_DISP, DVD_VIS_RGB = 0, 1, 2
 DVD_VIS_MAX_PANELS = 4
 
+
+class VisMap(ctypes.Structure):
+    """struct dvd_vis_map (include/dvd_b200.h)."""
+    _fields_ = [('src', ctypes.c_void_p), ('s_n', ctypes.c_longlong), ('s_c', ctypes.c_longlong), ('s_y', ctypes.c_longlong),
+                ('s_x', ctypes.c_longlong), ('kind', ctypes.c_int), ('n', ctypes.c_int), ('range', ctypes.c_int), ('tile', ctypes.c_int)]
+
+
+DVD_VIS_MAP_DEPTH, DVD_VIS_MAP_FLOW, DVD_VIS_MAP_IMG = 0, 1, 2
+DVD_VIS_MAX_MAPS = 16
+
 _I, _F, _P = ctypes.c_int, ctypes.c_float, ctypes.c_void_p
 _L = ctypes.c_longlong
 
@@ -149,6 +159,8 @@ SIGNATURES = {
     'dvd_voxel_reduce_scratch_bytes': [_L],
     'dvd_voxel_reduce': [_P, _P, _P, _P, _P, _L, _L, _I, _P, _P, _P, _P, _P, ctypes.c_size_t, ctypes.POINTER(_L), _P],
     'dvd_vis_panels': [_P, _L, _I, _I, _I, ctypes.POINTER(VisPanel), _I, _P, _P, _P],
+    'dvd_vis_ranges': [ctypes.POINTER(VisMap), _I, _I, _I, _P, _P],
+    'dvd_vis_tiles': [ctypes.POINTER(VisMap), _I, _I, _I, _P, _P, _P, _P, _P],
 }
 DVD_MASKS_FLOWPAIR_U8 = 0
 DVD_MASKS_PAIRFILE_F32 = 1

@@ -39,7 +39,7 @@ int num_sms() {
 extern "C" const char* dvd_last_error(void) { return dvd::g_err; }
 extern "C" int dvd_version(void) { return 103; }
 /* sizes of the structs that cross the C ABI by pointer (which: 0 dvd_loss_cfg, 1 dvd_mlp_cfg, 2 dvd_conv_desc, 3 dvd_pack_item,
- * 4 dvd_vis_panel): a binding in another language checks its own layout against these */
+ * 4 dvd_vis_panel, 5 dvd_vis_map): a binding in another language checks its own layout against these */
 extern "C" long dvd_struct_size(int which) {
   switch (which) {
     case 0: return (long)sizeof(dvd_loss_cfg);
@@ -47,6 +47,7 @@ extern "C" long dvd_struct_size(int which) {
     case 2: return (long)sizeof(dvd_conv_desc);
     case 3: return (long)sizeof(dvd_pack_item);
     case 4: return (long)sizeof(dvd_vis_panel);
+    case 5: return (long)sizeof(dvd_vis_map);
     default: return -1;
   }
 }

@@ -210,6 +210,8 @@ class NetInterface(object):
             if reset_dataset is not None:
                 reset_dataset.reset()
             run(dataloader, steps, epoch, self._train_on_batch, True)
+            if getattr(self, 'visualizer', None) is not None:
+                self.visualizer.flush()    # the epoch's page images are on disk before the epoch counts as done
             if train_epoch_callback is not None:
                 train_epoch_callback(epoch)
             if dataloader_vali is not None:

@@ -422,7 +422,11 @@ class Model(NetInterface):
         outdir = join(self.full_logdir, 'visualize', 'epoch%04d_train' % epoch)
         makedirs(outdir, exist_ok=True)
         if self.global_rank == 0 and self.visualizer is not None:
-            self.visualizer.visualize(out, indx + (1000 * epoch), outdir)
+            # the page images are rendered from the device tensors the npz arrays above were copied from
+            dev = dict(pred, img_1=inp.img_1, img_2=inp.img_2, flow_1_2=inp.flow_1_2, flow_2_1=inp.flow_2_1)
+            if 'depth_pred_1' in batch:
+                dev['depth_nn_1'] = batch['depth_pred_1'].to(self.device)
+            self.visualizer.visualize(dev, indx + (1000 * epoch), outdir)
         np.savez(join(outdir, 'rank%04d_batch%04d' % (self.global_rank, batch_ind)), **out)
 
     # ---- eval / test forward (smf.py:265-276; video_base.py:66-103,128-155) ---------------------------------
@@ -459,7 +463,7 @@ class Model(NetInterface):
         gt = batch['depth_mvs'].to(pred['depth'].device)
         return {'size': batch['img'].shape[0], 'loss': self.disp_vali(pred['depth'], gt).item()}
 
-    def validate_sequence(self, frames, batch_size=1, chunk=8):
+    def validate_sequence(self, frames, batch_size=1, chunk=8, epoch=None):
         """The reference's validation pass (train.py:234,319-346 with `_vali_on_batch`) over a device-resident sequence.
 
         `frames` holds the `vali` items of the dataset stacked along dim 0 (at least 'img' [F,3,H,W] and 'depth_mvs'
@@ -469,7 +473,10 @@ class Model(NetInterface):
 
         Returns the reference's `loss_eval`: the size-weighted mean of the per-batch `disp_vali` losses, i.e. the mean per-frame
         MSE over the frames of the complete batches. The step graphs, the MLP's wgmma pack and the nets' train / eval modes are
-        left as they were."""
+        left as they were.
+
+        With `epoch` given and a visualizer set, the first `vis_batches_vali` batches of an epoch with epoch % vis_every_vali
+        == 0 are also handled as the reference's `_vali_on_batch` visualises them (`_vali_visual`), after the loss."""
         img, gt = frames['img'], frames['depth_mvs']
         n = (img.shape[0] // batch_size) * batch_size
         if n < 1:
@@ -488,12 +495,29 @@ class Model(NetInterface):
                     x = img[s:e]
                     depth = self.net_depth(x) if self.opt.midas else self.net_depth(x, None)
                     ops.disp_vali(depth.contiguous(), gt[s:e].float().contiguous(), out=sse[s:e])
+            vis_every = getattr(self.opt, 'vis_every_vali', 0)
+            if epoch is not None and self.visualizer is not None and vis_every and epoch % vis_every == 0 and self.full_logdir:
+                for bi in range(min(getattr(self.opt, 'vis_batches_vali', 0), n // batch_size)):
+                    s, e = bi * batch_size, (bi + 1) * batch_size
+                    self._vali_visual(epoch, bi, {k: v[s:e] for k, v in frames.items() if torch.is_tensor(v) or isinstance(v, list)})
+                self.visualizer.flush()
         finally:
             for net, m in zip(self._nets, modes):
                 net.train(m)
         per_frame = sse.cpu().double() / float(H * W)      # the one read-back of the pass
         batch_losses = per_frame.reshape(-1, batch_size).mean(1)
         return float(batch_losses.mean())
+
+    def _vali_visual(self, epoch, batch_idx, batch):
+        """video_base.py:89-99: the page images and `rank%04d_batch%04d.npz` of one validation batch (device tensors)."""
+        self.load_batch(batch)
+        pred = self._predict_on_batch(is_train=False)
+        outdir = join(self.full_logdir, 'visualize', 'epoch%04d_vali' % epoch)
+        makedirs(outdir, exist_ok=True)
+        dev = dict(pred, img_1=batch['img'], img_2=batch['img'], depth_nn=batch['depth_pred'], depth_gt=batch['depth_mvs'].float())
+        self.visualizer.visualize(dev, batch_idx + (1000 * epoch), outdir)
+        out = self.pack_output({k: v.cpu().numpy() for k, v in pred.items()}, batch)
+        np.savez(join(outdir, 'rank%04d_batch%04d' % (self.global_rank, batch_idx)), **out)
 
     def pack_output(self, pred_all, batch):
         """video_base.py:105-126 for the per-frame (`img`) batches of the test pass."""

@@ -957,3 +957,53 @@ def vis_panels(tmpl, panels, lut, out, tmpl_stride=0):
     _lib.check(_lib.load().dvd_vis_panels(_ptr(tmpl), tmpl_stride, n, CH, CW, arr, len(panels), _ptr(lut if mapped else None),
                                           _ptr(out), _stream()), 'dvd_vis_panels')
     return out
+
+
+# ---- training / validation page images (csrc/train_vis.cu) ----------------------------------------------------------------------
+VIS_MAP_KINDS = {'depth': (_lib.DVD_VIS_MAP_DEPTH, 1), 'flow': (_lib.DVD_VIS_MAP_FLOW, 2), 'img': (_lib.DVD_VIS_MAP_IMG, 3)}
+
+
+def vis_map_array(maps, turbo, wheel):
+    """The checked host array of struct dvd_vis_map for `vis_tiles`: (array, H, W, number of tiles)."""
+    if not 1 <= len(maps) <= _lib.DVD_VIS_MAX_MAPS:
+        raise ValueError('1 to %d maps per call, got %d' % (_lib.DVD_VIS_MAX_MAPS, len(maps)))
+    for name, t, shape in (('turbo', turbo, (256, 3)), ('wheel', wheel, (55, 3))):
+        _chk_dtype(t, name, torch.float64, 2)
+        if tuple(t.shape) != shape:
+            raise ValueError('%s must be %s, got %s' % (name, shape, tuple(t.shape)))
+    H = W = None
+    arr = (_lib.VisMap * len(maps))()
+    n_tiles = 0
+    for q, (kind, src) in enumerate(maps):
+        if kind not in VIS_MAP_KINDS:
+            raise ValueError('maps[%d]: kind must be one of %s, got %r' % (q, sorted(VIS_MAP_KINDS), kind))
+        code, chans = VIS_MAP_KINDS[kind]
+        if not isinstance(src, torch.Tensor) or not src.is_cuda or src.dtype != torch.float32:
+            raise ValueError('maps[%d] must be a float32 CUDA tensor' % q)
+        if src.dim() != 4 or src.shape[1] != chans or min(src.stride()) < 0 or src.numel() == 0:
+            raise ValueError('maps[%d]: a %s map must be a non-empty [n,%d,H,W] view, got %s' % (q, kind, chans, tuple(src.shape)))
+        if H is None:
+            H, W = int(src.shape[2]), int(src.shape[3])
+        if (src.shape[2], src.shape[3]) != (H, W) or src.device != turbo.device or wheel.device != turbo.device:
+            raise ValueError('maps[%d]: every map of a call has the same H x W (%dx%d) and device, got %s' % (q, H, W, tuple(src.shape)))
+        n = int(src.shape[0])
+        arr[q] = _lib.VisMap(src.data_ptr(), *src.stride(), code, n, 2 * n_tiles, n_tiles)
+        n_tiles += n
+    return arr, H, W, n_tiles
+
+
+def vis_tiles(maps, turbo, wheel):
+    """dvd_vis_ranges + dvd_vis_tiles: the uint8 RGB tiles [T,H,W,3] of `maps`, a list of (kind, src) with kind 'depth', 'flow'
+    or 'img' and src an fp32 CUDA tensor indexed (image, channel, y, x) - any strides, so `flow.permute(0, 3, 1, 2)` of a
+    [B,H,W,2] flow is read in place. The tiles of map q follow those of maps 0..q-1, one per image. turbo: [256,3] fp64 RGB
+    colour table, wheel: [55,3] fp64 flow colour wheel over 255, both contiguous on the maps' device."""
+    arr, H, W, n_tiles = vis_map_array(maps, turbo, wheel)
+    dev = turbo.device
+    ranges = torch.empty(2 * n_tiles, dtype=torch.float32, device=dev)
+    tiles = torch.empty(n_tiles, H, W, 3, dtype=torch.uint8, device=dev)
+    lib = _lib.load()
+    LAUNCHES['n'] += 2
+    _lib.check(lib.dvd_vis_ranges(arr, len(maps), H, W, _ptr(ranges), _stream()), 'dvd_vis_ranges')
+    _lib.check(lib.dvd_vis_tiles(arr, len(maps), H, W, _ptr(ranges), _ptr(turbo), _ptr(wheel), _ptr(tiles), _stream()),
+               'dvd_vis_tiles')
+    return tiles

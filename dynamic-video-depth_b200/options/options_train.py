@@ -1,6 +1,7 @@
 """Flag surface of the reference's options/options_train.py:23-189, kept name for name: general flags,
 then the dataset's and the model's own flags through their `add_arguments` (two-pass parse, :165-189).
-Flags that only drive out-of-scope subsystems (loggers, html, tensorboard) are accepted and ignored."""
+`--html_logger` writes the training and validation pages (dvd_b200/train_vis.py). The other flags that only drive
+out-of-scope subsystems (CSV / TensorBoard loggers, `--vis_workers`, `--vis_param_f`) are accepted and ignored."""
 import argparse
 import sys
 

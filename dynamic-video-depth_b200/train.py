@@ -47,7 +47,7 @@ class _Validator:
         self.loss_eval = {}
 
     def __call__(self, epoch):
-        v = self.model.validate_sequence(self.frames, batch_size=self.batch_size)
+        v = self.model.validate_sequence(self.frames, batch_size=self.batch_size, epoch=epoch)
         self.loss_eval[epoch] = v
         if self.best_path and (self.best is None or v < self.best):
             self.best = v
@@ -120,6 +120,9 @@ def main_worker(local_rank, ngpus, opt):
                                              num_workers=opt.workers, pin_memory=True, drop_last=True)
 
     validator = _Validator(opt, model, Dataset, device) if (opt.validate and rank == 0) else None
+    if opt.html_logger and rank == 0 and opt.full_logdir:
+        from .train_vis import PageWriter
+        model.visualizer = PageWriter(opt.full_logdir)
 
     def on_epoch(epoch):
         if sampler is not None:
@@ -132,10 +135,14 @@ def main_worker(local_rank, ngpus, opt):
                                   additional_values={'epoch': epoch})
         if validator is not None:
             validator(epoch)
-    if validator is not None and opt.vali_at_start:
-        validator(initial_epoch - 1)
-    model.train_epoch(loader, epochs=opt.epoch, initial_epoch=initial_epoch, max_batches_per_train=opt.epoch_batches,
-                      global_rank=rank, train_epoch_callback=on_epoch)
+    try:
+        if validator is not None and opt.vali_at_start:
+            validator(initial_epoch - 1)
+        model.train_epoch(loader, epochs=opt.epoch, initial_epoch=initial_epoch, max_batches_per_train=opt.epoch_batches,
+                          global_rank=rank, train_epoch_callback=on_epoch)
+    finally:
+        if model.visualizer is not None:
+            model.visualizer.close()     # every page image is written (or its failure raised) before the run ends
     if rank == 0 and validator is None:
         for e, log in logger.epoch_logs:
             print('epoch %d:' % e, {k: round(v, 6) for k, v in log.items()})

@@ -45,8 +45,8 @@ enum { DVD_S_FLOW = 0, DVD_S_DISP = 1, DVD_S_SF = 2, DVD_S_LOSS = 3, DVD_S_MASKS
 
 const char* dvd_last_error(void);
 int dvd_version(void);
-/* sizeof of the structs passed by pointer: 0 dvd_loss_cfg, 1 dvd_mlp_cfg, 2 dvd_conv_desc, 3 dvd_pack_item, 4 dvd_vis_panel
- * (-1 otherwise) */
+/* sizeof of the structs passed by pointer: 0 dvd_loss_cfg, 1 dvd_mlp_cfg, 2 dvd_conv_desc, 3 dvd_pack_item, 4 dvd_vis_panel,
+ * 5 dvd_vis_map (-1 otherwise) */
 long dvd_struct_size(int which);
 /* number of fp32 partial-sum slots dvd_reproject_loss_fwd needs in `partials` for a given shape */
 int dvd_reproject_partials_size(int B, int H, int W);
@@ -430,6 +430,31 @@ typedef struct dvd_vis_panel {
  * One thread writes 8 consecutive pixels of a row; every output byte is written once, no atomics.                             */
 int dvd_vis_panels(const unsigned char* tmpl, long long tmpl_stride, int n_canvas, int CH, int CW, const dvd_vis_panel* panels,
                    int n_panels, const unsigned char* lut, unsigned char* out, void* stream);
+
+/* ---- training / validation pages (csrc/train_vis.cu): the images of util/util_visualize.py and util/util_flow.py as the
+ * reference's HTMLVisualizer writes them for one visualised pack. ------------------------------------------------------------ */
+#define DVD_VIS_MAX_MAPS 16
+enum { DVD_VIS_MAP_DEPTH = 0, DVD_VIS_MAP_FLOW = 1, DVD_VIS_MAP_IMG = 2 };
+/* One image key of a pack: n images of H x W, element (i, c, y, x) at src[i s_n + c s_c + y s_y + x s_x] (strides in elements,
+ * so a permuted view such as [B,2,H,W].permute(0,2,3,1) is read in place). c is 0 for DEPTH, 0 / 1 (u / v) for FLOW and 0..2
+ * (R, G, B) for IMG. Image i uses the fp32 pair ranges[range + 2 i], ranges[range + 2 i + 1] and writes tile `tile + i`.       */
+typedef struct dvd_vis_map {
+  const float* src;
+  long long s_n, s_c, s_y, s_x;
+  int kind;
+  int n;
+  int range;
+  int tile;
+} dvd_vis_map;
+/* Per image of each map, exact fp32 extrema with NaN propagating (np.min / np.max): DEPTH min, max of t = 1 / (d + 1e-6f);
+ * FLOW max of rad = sqrt(u u + v v) after |u| or |v| > 1e7 zeroes both (the second slot repeats it); IMG min, max over the
+ * three channels (dvd_vis_tiles folds them over the map's n images). One CTA per image, no atomics.                           */
+int dvd_vis_ranges(const dvd_vis_map* maps, int n_maps, int H, int W, float* ranges, void* stream);
+/* tiles [*, H, W, 3] uint8 RGB, from the ranges dvd_vis_ranges wrote. turbo: [256, 3] fp64 colour table in [0, 1]; wheel:
+ * [55, 3] fp64 Middlebury colour wheel over 255. The rules and their dtypes are spelled out in csrc/train_vis.cu. `maps` is a
+ * HOST array of n_maps <= DVD_VIS_MAX_MAPS maps (-1 otherwise). One thread writes 4 consecutive pixels of a row, no atomics. */
+int dvd_vis_tiles(const dvd_vis_map* maps, int n_maps, int H, int W, const float* ranges, const double* turbo, const double* wheel,
+                  unsigned char* tiles, void* stream);
 
 /* ---- RAFT optical flow, forward only (csrc/raft_ops.cu): third_party/RAFT/core as scripts/preprocess/davis/generate_flows.py runs it
  * (large model, all-pairs correlation, 4 levels, radius 4, hidden = context = 128, no warm start, test_mode). These are the CUDA-core
