@@ -125,6 +125,22 @@ SIGNATURES = {
                        ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float), _P, _I, _I, _I, _P],
     'dvd_head_fwd': [_P, _P, _P, _P, ctypes.c_long, _P],
     'dvd_head_bwd': [_P, _P, _P, _P, _P, _P, _P, ctypes.c_long, _I, _I, _P],
+    'dvd_ordered_workspace_bytes': [_I],
+    'dvd_reproject_ordered_bytes': [_I, _I, _I],
+    'dvd_conv2d_wgrad_ordered': [ctypes.POINTER(ConvDesc), _P, _P, _P, _P, ctypes.c_long, ctypes.c_long, ctypes.c_long,
+                                 ctypes.c_long, _I, _I, _P, _P, _P, _P, _P, _P, ctypes.c_size_t, _P],
+    'dvd_mlp_wgrad_ordered': [ctypes.POINTER(MlpCfg), _P, _P, ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_void_p),
+                              ctypes.c_long, _P, ctypes.c_size_t, _P],
+    'dvd_mlp_dgrad_ordered': [ctypes.POINTER(MlpCfg), _P, _P, _P, _F, _I, _I, _P, _P, _P, _P, _P, _P, _P,
+                              ctypes.c_long, ctypes.c_long, _P, ctypes.c_size_t, _P],
+    'dvd_reproject_loss_bwd_ordered': [_P, _P, _P, _P, _P, _P, ctypes.POINTER(LossCfg), _P, _F, _P, _P, _P, _I, _I, _I, _P,
+                                       ctypes.c_size_t, _P],
+    'dvd_relu_bwd_colsum_ordered': [_P, _P, _P, _P, _P, _P, _F, _P, ctypes.c_long, _I, _I, _P, ctypes.c_size_t, _P],
+    'dvd_bn_act_bwd_ordered': [_P, _P, _P, _P, _P, _P, _F, _P, _P, _P, _P, ctypes.c_long, _I, _I, _P, ctypes.c_size_t, _P],
+    'dvd_stem_wgrad_ordered': [_P, _P, _P, _P, _P, ctypes.c_long, ctypes.c_long, ctypes.c_long, ctypes.c_long, _P, _P, _P, _F,
+                               _P, _P, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float), _P, _I, _I, _I, _P,
+                               ctypes.c_size_t, _P],
+    'dvd_head_bwd_ordered': [_P, _P, _P, _P, _P, _P, _P, ctypes.c_long, _I, _I, _P, ctypes.c_size_t, _P],
     'dvd_flow_resize_cubic': [_P, ctypes.c_size_t, _P, ctypes.c_size_t, _I, _I, _I, _I, _I, _P],
     'dvd_flow_pair_masks': [_P, _P, ctypes.c_size_t, _P, _P, ctypes.c_size_t, _I, _I, _I, _I, _P],
     'dvd_disp_vali_partials_size': [_I, _I, _I],
@@ -168,7 +184,11 @@ _RESTYPES = {'dvd_last_error': ctypes.c_char_p, 'dvd_struct_size': ctypes.c_long
              'dvd_mlp_save_bytes_per_eval': ctypes.c_size_t, 'dvd_mlp_dy_bytes': ctypes.c_size_t,
              'dvd_raft_instnorm_scratch_bytes': ctypes.c_long, 'dvd_raft_pyramid_floats': ctypes.c_long,
              'dvd_aa_resize_scratch_bytes': ctypes.c_long, 'dvd_points_select_scratch_bytes': ctypes.c_long,
-             'dvd_voxel_reduce_scratch_bytes': ctypes.c_long}
+             'dvd_voxel_reduce_scratch_bytes': ctypes.c_long, 'dvd_ordered_workspace_bytes': ctypes.c_size_t,
+             'dvd_reproject_ordered_bytes': ctypes.c_size_t}
+
+# sites of dvd_ordered_workspace_bytes (include/dvd_b200.h)
+DVD_ORD_CONV_WGRAD, DVD_ORD_MLP_WGRAD, DVD_ORD_MLP_DGRAD, DVD_ORD_CHANNEL_SUMS, DVD_ORD_STEM, DVD_ORD_HEAD = range(6)
 
 _lib = None
 

@@ -11,7 +11,7 @@ import torch
 
 from . import _lib
 from ._lib import ConvDesc, DVD_CONV_MAX_TAPS
-from .ops import LAUNCHES, _ptr, _stream
+from .ops import LAUNCHES, _ptr, _stream, _ws, ordered, ordered_workspace
 
 GROUP_BLOCK = 64     # grouped convolutions run as block-diagonal GEMM blocks of this many channels
 
@@ -218,9 +218,16 @@ def wgrad_launch(desc, x, gy, dweight, ksize, groups=1, weight=None, bn=None, dg
     g, v = bn if bn is not None else (None, None)
     LAUNCHES['n'] += 1
     ev = _prof('wgrad', flops, desc)
-    _lib.check(_lib.load().dvd_conv2d_wgrad(ctypes.byref(desc), _ptr(x), _ptr(gy), _ptr(dweight), _ptr(weight), st[0], st[1], st[2],
-                                            st[3], int(ksize), int(groups), _ptr(g), _ptr(v), _ptr(dgamma), _ptr(colsum), _ptr(bn_mean),
-                                            _stream()), 'dvd_conv2d_wgrad')
+    if ordered():
+        LAUNCHES['n'] += 2
+        ws = _ws(ordered_workspace(dweight.device, _lib.DVD_ORD_CONV_WGRAD))
+        _lib.check(_lib.load().dvd_conv2d_wgrad_ordered(ctypes.byref(desc), _ptr(x), _ptr(gy), _ptr(dweight), _ptr(weight), st[0], st[1],
+                                                        st[2], st[3], int(ksize), int(groups), _ptr(g), _ptr(v), _ptr(dgamma),
+                                                        _ptr(colsum), _ptr(bn_mean), *ws, _stream()), 'dvd_conv2d_wgrad_ordered')
+    else:
+        _lib.check(_lib.load().dvd_conv2d_wgrad(ctypes.byref(desc), _ptr(x), _ptr(gy), _ptr(dweight), _ptr(weight), st[0], st[1], st[2],
+                                                st[3], int(ksize), int(groups), _ptr(g), _ptr(v), _ptr(dgamma), _ptr(colsum),
+                                                _ptr(bn_mean), _stream()), 'dvd_conv2d_wgrad')
     if ev is not None:
         ev.record()
 
@@ -230,6 +237,13 @@ def relu_bwd_colsum(g, y=None, gm=None, colsum=None, bn=None, dgamma=None, round
     N, C, H, W = g.shape
     m, v, eps = bn if bn is not None else (None, None, 0.0)
     LAUNCHES['n'] += 1
+    if ordered() and (colsum is not None or dgamma is not None):
+        LAUNCHES['n'] += 1
+        ws = _ws(ordered_workspace(g.device, _lib.DVD_ORD_CHANNEL_SUMS))
+        _lib.check(_lib.load().dvd_relu_bwd_colsum_ordered(_ptr(g), _ptr(y), _ptr(gm), _ptr(colsum), _ptr(m), _ptr(v), float(eps),
+                                                           _ptr(dgamma), N * H * W, C, int(bool(round_out)), *ws, _stream()),
+                   'dvd_relu_bwd_colsum_ordered')
+        return gm
     _lib.check(_lib.load().dvd_relu_bwd_colsum(_ptr(g), _ptr(y), _ptr(gm), _ptr(colsum), _ptr(m), _ptr(v), float(eps), _ptr(dgamma),
                                                N * H * W, C, int(bool(round_out)), _stream()), 'dvd_relu_bwd_colsum')
     return gm
@@ -279,10 +293,15 @@ def stem_wgrad(x_nchw, g, a0, conv, bn, norm_mean=None, norm_std=None):
         raise ValueError('parameter and gradient must share their strides')
     scratch = torch.empty(147 * 64 + 64, dtype=torch.float32, device=g.device)
     LAUNCHES['n'] += 3
-    _lib.check(_lib.load().dvd_stem_wgrad(_ptr(x_nchw), _ptr(g), _ptr(a0), _ptr(conv.weight), _ptr(conv.weight.grad), st[0], st[1],
-                                          st[2], st[3], _ptr(bn.weight), _ptr(bn.running_mean), _ptr(bn.running_var), float(bn.eps),
-                                          _ptr(bn.weight.grad), _ptr(bn.bias.grad), _f3(norm_mean), _f3(norm_std), _ptr(scratch),
-                                          N, H, W, _stream()), 'dvd_stem_wgrad')
+    args = (_ptr(x_nchw), _ptr(g), _ptr(a0), _ptr(conv.weight), _ptr(conv.weight.grad), st[0], st[1], st[2], st[3], _ptr(bn.weight),
+            _ptr(bn.running_mean), _ptr(bn.running_var), float(bn.eps), _ptr(bn.weight.grad), _ptr(bn.bias.grad), _f3(norm_mean),
+            _f3(norm_std), _ptr(scratch), N, H, W)
+    if ordered():
+        LAUNCHES['n'] += 1
+        ws = _ws(ordered_workspace(g.device, _lib.DVD_ORD_STEM))
+        _lib.check(_lib.load().dvd_stem_wgrad_ordered(*args, *ws, _stream()), 'dvd_stem_wgrad_ordered')
+    else:
+        _lib.check(_lib.load().dvd_stem_wgrad(*args, _stream()), 'dvd_stem_wgrad')
 
 
 def head_fwd(x, weight, bias):
@@ -300,8 +319,14 @@ def head_bwd(x, weight, bias, g_depth, gw, gb, relu_mask=True, round_out=True):
     N, C, H, W = x.shape
     gx = torch.empty_like(x)
     LAUNCHES['n'] += 1
-    _lib.check(_lib.load().dvd_head_bwd(_ptr(x), _ptr(weight), _ptr(bias), _ptr(g_depth), _ptr(gx), _ptr(gw), _ptr(gb), N * H * W,
-                                        int(bool(relu_mask)), int(bool(round_out)), _stream()), 'dvd_head_bwd')
+    args = (_ptr(x), _ptr(weight), _ptr(bias), _ptr(g_depth), _ptr(gx), _ptr(gw), _ptr(gb), N * H * W, int(bool(relu_mask)),
+            int(bool(round_out)))
+    if ordered():
+        LAUNCHES['n'] += 1
+        ws = _ws(ordered_workspace(x.device, _lib.DVD_ORD_HEAD))
+        _lib.check(_lib.load().dvd_head_bwd_ordered(*args, *ws, _stream()), 'dvd_head_bwd_ordered')
+    else:
+        _lib.check(_lib.load().dvd_head_bwd(*args, _stream()), 'dvd_head_bwd')
     return gx
 
 

@@ -74,6 +74,13 @@ __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepc
     dvd::pdl_launch_dependents();  \
   } while (0)
 
+// ---- ordered reductions (DESIGN.md 2.11) ----------------------------------------------------------------------------
+// The *_ordered entry points do not add partial sums into shared outputs with fp32 atomics, whose order changes from run to
+// run: every CTA (or warp) writes its partials into a slab of its own in a caller-supplied workspace, and ordered_sum adds the
+// slabs in slab order: dst0[i] += sum_s slab[s * n + i] for i < n0, dst1[i - n0] += ... for n0 <= i < n (dst1 may be null
+// when n0 == n).
+int launch_ordered_sum(const float* slab, int nslab, long n, float* dst0, long n0, float* dst1, cudaStream_t st);
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -461,9 +461,22 @@ struct WgradParams {
   const float* mean;               // with colsum and dgamma: dgamma[m] -= mean[m] * rstd[m] * colsum[m]
   signed char dy[DVD_CONV_MAX_TAPS], dx[DVD_CONV_MAX_TAPS];
   unsigned char wt[DVD_CONV_MAX_TAPS];
+  // ordered variant: per-CTA slabs of the partial tiles ([128 rows][NT columns], ksplit > 1 only) and of the rows
+  // ([0, 128): dgamma partial, [128, 256): column-sum partial)
+  float* ord_tiles;
+  float* ord_rows;
 };
 
-template <int NT, bool G64>
+// the CTA's output tile: tap t, first M channel m0, first N channel n0
+struct WgTile { int t, m0, n0; };
+__device__ __forceinline__ WgTile wgrad_tile(const WgradParams& P, int NT, int out_grp) {
+  const int n_m = P.Mch / 128, n_n = P.cpg ? 1 : P.Nch / NT;
+  const int t = out_grp / (n_m * n_n), rem = out_grp - t * (n_m * n_n);
+  const int m0 = (rem / n_n) * 128;
+  return {t, m0, P.cpg ? m0 : (rem % n_n) * NT};
+}
+
+template <int NT, bool G64, bool ORD = false>
 __global__ void __launch_bounds__(kWgThreads, 1) conv_wgrad_kernel(const __grid_constant__ CUtensorMap mapM,
                                                                   const __grid_constant__ CUtensorMap mapN,
                                                                   const __grid_constant__ WgradParams P) {
@@ -625,6 +638,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) conv_wgrad_kernel(const __grid_
       cs[h] += __shfl_xor_sync(0xffffffffu, cs[h], 2);
     }
   }
+  if constexpr (!ORD) {
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int lm = lrow + 8 * h, m = m0 + lm;
@@ -659,6 +673,88 @@ __global__ void __launch_bounds__(kWgThreads, 1) conv_wgrad_kernel(const __grid_
       }
       if (P.dgamma) atomicAdd(P.dgamma + m, dot * rstd);
     }
+  }
+  } else {
+    // The tile goes to this CTA's slab (conv_wgrad_tile_reduce_kernel adds the slabs of a tile in split order) or, when the
+    // pixels are not split, straight into dw: no other CTA of the launch writes these elements. dgamma and column-sum
+    // partials go to the row slab (conv_wgrad_row_reduce_kernel).
+    float* tile = P.ord_tiles + (size_t)blockIdx.x * (128 * NT);
+    float* rows = P.ord_rows + (size_t)blockIdx.x * 256;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int lm = lrow + 8 * h, m = m0 + lm;
+      float* dst = P.dw + (long)m * P.s_m + tap_off;
+      const float* wrow = P.w ? P.w + (long)m * P.s_m + tap_off : nullptr;
+      float sc = 1.f, rstd = 0.f;
+      if (P.gamma) {
+        rstd = rsqrtf(__ldg(P.var + m) + P.eps);
+        sc = __ldg(P.gamma + m) * rstd;
+      }
+      float dot = 0.f;
+#pragma unroll
+      for (int j = 0; j < WN / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int ln = noff + j * 8 + 2 * tq + e;
+          if (P.cpg && ln / P.cpg != lm / P.cpg) continue;
+          const long o = (long)(P.cpg ? ln % P.cpg : n0 + ln) * P.s_n;
+          const float v = acc[4 * j + 2 * h + e];
+          if (wrow) dot = fmaf(v, __ldg(wrow + o), dot);
+          if (P.ksplit == 1) dst[o] += v * sc;
+          else tile[lm * NT + ln] = v * sc;
+        }
+      }
+      if (P.dgamma) {
+        dot += __shfl_xor_sync(0xffffffffu, dot, 1);
+        dot += __shfl_xor_sync(0xffffffffu, dot, 2);
+      }
+      if (tq == 0) {
+        if (do_colsum) {
+          rows[128 + lm] = cs[h];
+          if (P.dgamma && P.mean) dot = fmaf(-__ldg(P.mean + m), cs[h], dot);
+        }
+        if (P.dgamma) rows[lm] = dot * rstd;
+      }
+    }
+  }
+}
+
+// dw[tile element] += the tile's split partials in split order (nparts: the splits with a non-empty pixel range)
+__global__ void __launch_bounds__(256) conv_wgrad_tile_reduce_kernel(const __grid_constant__ WgradParams P, int NT, int nparts,
+                                                                     long n) {
+  DVD_PDL_ENTER();
+  const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n) return;
+  const int out_grp = (int)(idx / (128 * NT)), r = (int)(idx - (long)out_grp * 128 * NT), lm = r / NT, ln = r - lm * NT;
+  if (P.cpg && ln / P.cpg != lm / P.cpg) return;
+  const WgTile T = wgrad_tile(P, NT, out_grp);
+  const int wt = P.wt[T.t];
+  const long o = (long)(T.m0 + lm) * P.s_m + (long)(wt / P.ksize) * P.s_ky + (long)(wt % P.ksize) * P.s_kx +
+                 (long)(P.cpg ? ln % P.cpg : T.n0 + ln) * P.s_n;
+  const float* src = P.ord_tiles + (size_t)out_grp * P.ksplit * (128 * NT) + r;
+  float s = 0.f;
+  for (int p = 0; p < nparts; ++p) s += __ldcg(src + (size_t)p * (128 * NT));
+  P.dw[o] += s;
+}
+
+// colsum[m] += its partials in split order; dgamma[m] += its partials in (tap, N tile, split) order
+__global__ void __launch_bounds__(128) conv_wgrad_row_reduce_kernel(const __grid_constant__ WgradParams P, int NT, int nparts) {
+  DVD_PDL_ENTER();
+  const int m = blockIdx.x * 128 + threadIdx.x, mb = blockIdx.x, lm = threadIdx.x;
+  const int n_m = P.Mch / 128, n_n = P.cpg ? 1 : P.Nch / NT;
+  if (P.colsum) {
+    float s = 0.f;
+    for (int p = 0; p < nparts; ++p) s += __ldcg(P.ord_rows + (size_t)(mb * n_n * P.ksplit + p) * 256 + 128 + lm);
+    P.colsum[m] += s;
+  }
+  if (P.dgamma) {
+    float s = 0.f;
+    for (int t = 0; t < P.ntaps; ++t)
+      for (int nt = 0; nt < n_n; ++nt) {
+        const int out_grp = (t * n_m + mb) * n_n + nt;
+        for (int p = 0; p < nparts; ++p) s += __ldcg(P.ord_rows + (size_t)(out_grp * P.ksplit + p) * 256 + lm);
+      }
+    P.dgamma[m] += s;
   }
 }
 
@@ -751,7 +847,8 @@ int launch_conv(const CUtensorMap& mapA, const CUtensorMap& mapW, const ConvPara
 }
 
 template <int NT, bool G64>
-int launch_wgrad(const CUtensorMap& mapM, const CUtensorMap& mapN, WgradParams P, int out_tiles, int px_tiles, cudaStream_t st) {
+int launch_wgrad(const CUtensorMap& mapM, const CUtensorMap& mapN, WgradParams P, int out_tiles, int px_tiles, cudaStream_t st,
+                 void* ws = nullptr, size_t ws_bytes = 0) {
   static bool attr_done[16] = {};
   if (int e = per_device_attr((const void*)conv_wgrad_kernel<NT, G64>, kWgSmem, attr_done)) return e;
   // split-K so that all CTAs are resident in ONE wave (a second, nearly empty wave would double the time)
@@ -760,8 +857,34 @@ int launch_wgrad(const CUtensorMap& mapM, const CUtensorMap& mapN, WgradParams P
   if (ksplit > px_tiles) ksplit = px_tiles;
   if (ksplit < 1) ksplit = 1;
   P.ksplit = ksplit;
-  DVD_CUDA_CALL(dvd::launch(conv_wgrad_kernel<NT, G64>, out_tiles * ksplit, kWgThreads, kWgSmem, st, mapM, mapN, P));
-  DVD_CUDA_LAUNCH_CHECK("conv_wgrad_kernel");
+  if (ws == nullptr) {
+    DVD_CUDA_CALL(dvd::launch(conv_wgrad_kernel<NT, G64>, out_tiles * ksplit, kWgThreads, kWgSmem, st, mapM, mapN, P));
+    DVD_CUDA_LAUNCH_CHECK("conv_wgrad_kernel");
+    return 0;
+  }
+  // ordered: the same split, partials through the workspace (DVD_ORD_CONV_WGRAD layout: tile slabs, then row slabs)
+  static bool attr_done_ord[16] = {};
+  if (int e = per_device_attr((const void*)conv_wgrad_kernel<NT, G64, true>, kWgSmem, attr_done_ord)) return e;
+  const int grid = out_tiles * ksplit;
+  const size_t tile_floats = (size_t)num_sms() * 128 * 256;
+  DVD_ARG_CHECK(ws_bytes >= dvd_ordered_workspace_bytes(DVD_ORD_CONV_WGRAD) && aligned16(ws),
+                "ordered weight gradient: the workspace needs dvd_ordered_workspace_bytes(DVD_ORD_CONV_WGRAD) bytes, 16-byte aligned");
+  DVD_ARG_CHECK(ksplit == 1 || (size_t)grid * 128 * NT <= tile_floats, "ordered weight gradient: %d split CTAs exceed the workspace", grid);
+  DVD_ARG_CHECK(grid <= DVD_ORD_CONV_MAX_CTAS, "ordered weight gradient: %d CTAs exceed DVD_ORD_CONV_MAX_CTAS", grid);
+  P.ord_tiles = (float*)ws;
+  P.ord_rows = (float*)ws + tile_floats;
+  DVD_CUDA_CALL(dvd::launch(conv_wgrad_kernel<NT, G64, true>, grid, kWgThreads, kWgSmem, st, mapM, mapN, P));
+  DVD_CUDA_LAUNCH_CHECK("conv_wgrad_kernel<ordered>");
+  const int per = (px_tiles + ksplit - 1) / ksplit, nparts = (px_tiles + per - 1) / per;
+  if (ksplit > 1) {
+    const long n = (long)out_tiles * 128 * NT;
+    DVD_CUDA_CALL(dvd::launch(conv_wgrad_tile_reduce_kernel, (unsigned)((n + 255) / 256), 256, 0, st, P, NT, nparts, n));
+    DVD_CUDA_LAUNCH_CHECK("conv_wgrad_tile_reduce_kernel");
+  }
+  if (P.dgamma || P.colsum) {
+    DVD_CUDA_CALL(dvd::launch(conv_wgrad_row_reduce_kernel, P.Mch / 128, 128, 0, st, P, NT, nparts));
+    DVD_CUDA_LAUNCH_CHECK("conv_wgrad_row_reduce_kernel");
+  }
   return 0;
 }
 
@@ -954,10 +1077,10 @@ extern "C" int dvd_conv2d_pack_batch(const dvd_pack_item* items_dev, int n_items
   return 0;
 }
 
-extern "C" int dvd_conv2d_wgrad(const dvd_conv_desc* desc, const float* x, const float* gy, float* dweight, const float* weight,
-                                long stride_co, long stride_ci, long stride_ky, long stride_kx, int ksize, int groups,
-                                const float* bn_gamma, const float* bn_var, float* dgamma, float* colsum, const float* bn_mean,
-                                void* stream) {
+static int conv2d_wgrad(const dvd_conv_desc* desc, const float* x, const float* gy, float* dweight, const float* weight,
+                        long stride_co, long stride_ci, long stride_ky, long stride_kx, int ksize, int groups,
+                        const float* bn_gamma, const float* bn_var, float* dgamma, float* colsum, const float* bn_mean,
+                        void* ws, size_t ws_bytes, void* stream) {
   DVD_ARG_CHECK(desc && x && gy && dweight, "null pointer");
   const dvd_conv_desc& d = *desc;
   DVD_ARG_CHECK(d.N >= 1 && d.H >= 1 && d.W >= 1 && d.OH >= 1 && d.OW >= 1, "bad shape");
@@ -1013,15 +1136,32 @@ extern "C" int dvd_conv2d_wgrad(const dvd_conv_desc* desc, const float* x, const
   const CUtensorMap& mapM = P.swap ? mapX : mapG;
   const CUtensorMap& mapN = P.swap ? mapG : mapX;
   const cudaStream_t st = (cudaStream_t)stream;
-  if (P.cpg && 64 % P.cpg == 0) return launch_wgrad<128, true>(mapM, mapN, P, out_tiles, px_tiles, st);
+  if (P.cpg && 64 % P.cpg == 0) return launch_wgrad<128, true>(mapM, mapN, P, out_tiles, px_tiles, st, ws, ws_bytes);
   switch (NT) {
-    case 32: return launch_wgrad<32, false>(mapM, mapN, P, out_tiles, px_tiles, st);
-    case 64: return launch_wgrad<64, false>(mapM, mapN, P, out_tiles, px_tiles, st);
-    case 96: return launch_wgrad<96, false>(mapM, mapN, P, out_tiles, px_tiles, st);
-    case 128: return launch_wgrad<128, false>(mapM, mapN, P, out_tiles, px_tiles, st);
-    case 160: return launch_wgrad<160, false>(mapM, mapN, P, out_tiles, px_tiles, st);
-    case 192: return launch_wgrad<192, false>(mapM, mapN, P, out_tiles, px_tiles, st);
-    case 224: return launch_wgrad<224, false>(mapM, mapN, P, out_tiles, px_tiles, st);
-    default: return launch_wgrad<256, false>(mapM, mapN, P, out_tiles, px_tiles, st);
+    case 32: return launch_wgrad<32, false>(mapM, mapN, P, out_tiles, px_tiles, st, ws, ws_bytes);
+    case 64: return launch_wgrad<64, false>(mapM, mapN, P, out_tiles, px_tiles, st, ws, ws_bytes);
+    case 96: return launch_wgrad<96, false>(mapM, mapN, P, out_tiles, px_tiles, st, ws, ws_bytes);
+    case 128: return launch_wgrad<128, false>(mapM, mapN, P, out_tiles, px_tiles, st, ws, ws_bytes);
+    case 160: return launch_wgrad<160, false>(mapM, mapN, P, out_tiles, px_tiles, st, ws, ws_bytes);
+    case 192: return launch_wgrad<192, false>(mapM, mapN, P, out_tiles, px_tiles, st, ws, ws_bytes);
+    case 224: return launch_wgrad<224, false>(mapM, mapN, P, out_tiles, px_tiles, st, ws, ws_bytes);
+    default: return launch_wgrad<256, false>(mapM, mapN, P, out_tiles, px_tiles, st, ws, ws_bytes);
   }
+}
+
+extern "C" int dvd_conv2d_wgrad(const dvd_conv_desc* desc, const float* x, const float* gy, float* dweight, const float* weight,
+                                long stride_co, long stride_ci, long stride_ky, long stride_kx, int ksize, int groups,
+                                const float* bn_gamma, const float* bn_var, float* dgamma, float* colsum, const float* bn_mean,
+                                void* stream) {
+  return conv2d_wgrad(desc, x, gy, dweight, weight, stride_co, stride_ci, stride_ky, stride_kx, ksize, groups, bn_gamma, bn_var,
+                      dgamma, colsum, bn_mean, nullptr, 0, stream);
+}
+
+extern "C" int dvd_conv2d_wgrad_ordered(const dvd_conv_desc* desc, const float* x, const float* gy, float* dweight,
+                                        const float* weight, long stride_co, long stride_ci, long stride_ky, long stride_kx,
+                                        int ksize, int groups, const float* bn_gamma, const float* bn_var, float* dgamma,
+                                        float* colsum, const float* bn_mean, void* ws, size_t ws_bytes, void* stream) {
+  DVD_ARG_CHECK(ws != nullptr, "dvd_conv2d_wgrad_ordered: null workspace");
+  return conv2d_wgrad(desc, x, gy, dweight, weight, stride_co, stride_ci, stride_ky, stride_kx, ksize, groups, bn_gamma, bn_var,
+                      dgamma, colsum, bn_mean, ws, ws_bytes, stream);
 }

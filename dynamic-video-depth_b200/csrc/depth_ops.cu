@@ -38,11 +38,12 @@ __global__ void __launch_bounds__(kThreads) round_kernel(const float4* __restric
 
 // gm = g * [y > 0]; colsum[c] += sum_p gm[p, c]; dgamma[c] -= mean[c] * rstd[c] * sum_p gm[p, c]
 // block = (cgb channel groups of 4) x (256 / cgb pixel rows); grid.x over pixel slabs, grid.y over channel blocks
+template <bool ORD = false>
 __global__ void __launch_bounds__(kThreads) relu_bwd_colsum_kernel(const float4* __restrict__ g, const float4* __restrict__ y,
                                                                    float4* __restrict__ gm, float* __restrict__ colsum,
                                                                    const float* __restrict__ mean, const float* __restrict__ var,
                                                                    float eps, float* __restrict__ dgamma, long P, int c4, int cgb,
-                                                                   int round_out) {
+                                                                   int round_out, float* __restrict__ ord) {
   DVD_PDL_ENTER();
   __shared__ float red[kThreads][4];
   const int tx = threadIdx.x % cgb, ty = threadIdx.x / cgb, rows = kThreads / cgb;
@@ -70,13 +71,31 @@ __global__ void __launch_bounds__(kThreads) relu_bwd_colsum_kernel(const float4*
     for (int r = 0; r < rows; ++r)
 #pragma unroll
       for (int k = 0; k < 4; ++k) a[k] += red[r * cgb + tx][k];
+    if constexpr (ORD) {      // ordered variant: [CTA column][channel] slab, added by colsum_ordered_reduce_kernel
+#pragma unroll
+      for (int k = 0; k < 4; ++k) ord[(size_t)blockIdx.x * 4 * c4 + cg * 4 + k] = a[k];
+    } else {
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const int c = cg * 4 + k;
       if (colsum) atomicAdd(colsum + c, a[k]);
       if (dgamma) atomicAdd(dgamma + c, -mean[c] * rsqrtf(var[c] + eps) * a[k]);
     }
+    }
   }
+}
+
+// s = sum of channel c's partials in CTA order; colsum[c] += s; dgamma[c] -= mean[c] * rstd[c] * s
+__global__ void __launch_bounds__(kThreads) colsum_ordered_reduce_kernel(const float* __restrict__ ord, int nb, int C,
+                                                                         float* colsum, const float* __restrict__ mean,
+                                                                         const float* __restrict__ var, float eps, float* dgamma) {
+  DVD_PDL_ENTER();
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  float s = 0.f;
+  for (int b = 0; b < nb; ++b) s += __ldcg(ord + (size_t)b * C + c);
+  if (colsum) colsum[c] += s;
+  if (dgamma) dgamma[c] += -mean[c] * rsqrtf(var[c] + eps) * s;
 }
 
 // ---- MaxPool2d(3, stride 2, padding 1), NHWC; idx = position (0..8) of the first maximum inside the window -----------
@@ -227,10 +246,11 @@ __global__ void __launch_bounds__(128) stem_fwd_kernel(const float* __restrict__
 
 // dWu[t][co] += sum_px gm[px][co] * xn[px, tap t];  gm = g * [a0 > 0];  bsum[co] += sum gm.   256 threads: thread owns the channel
 // quad (tid % 16) and the taps tid/16 + 16 i (i < 10), accumulated in registers over all tiles of the CTA, one atomic flush.
+template <bool ORD = false>
 __global__ void __launch_bounds__(256) stem_wgrad_kernel(const float* __restrict__ x, const float* __restrict__ g,
                                                          const float* __restrict__ a0, float3 nmean, float3 nrstd,
                                                          float* __restrict__ dwu, float* __restrict__ bsum, int N, int H, int W, int OH,
-                                                         int OW) {
+                                                         int OW, float* __restrict__ ord) {
   DVD_PDL_ENTER();
   __shared__ float patch[3][kStemPH][kStemPW];
   __shared__ __align__(16) float gsm[128][64];
@@ -281,6 +301,19 @@ __global__ void __launch_bounds__(256) stem_wgrad_kernel(const float* __restrict
       }
     }
   }
+  if constexpr (ORD) {        // ordered variant: this CTA's slab has the layout of (dwu, bsum); ordered_sum adds the slabs in CTA order
+    dwu = ord + (size_t)blockIdx.x * (kStemTaps * 64 + 64);
+#pragma unroll
+    for (int i = 0; i < 10; ++i) {
+      const int t = tg + 16 * i;
+      if (t < kStemTaps)
+#pragma unroll
+        for (int k = 0; k < 4; ++k) dwu[t * 64 + cq * 4 + k] = acc[i][k];
+    }
+    if (tg == 0)
+#pragma unroll
+      for (int k = 0; k < 4; ++k) dwu[kStemTaps * 64 + cq * 4 + k] = bs[k];
+  } else {
 #pragma unroll
   for (int i = 0; i < 10; ++i) {
     const int t = tg + 16 * i;
@@ -291,6 +324,7 @@ __global__ void __launch_bounds__(256) stem_wgrad_kernel(const float* __restrict
   if (tg == 0)
 #pragma unroll
     for (int k = 0; k < 4; ++k) atomicAdd(bsum + cq * 4 + k, bs[k]);
+  }
 }
 
 // dW[co] += sc[co] * dWu[co];  dgamma[co] += rstd[co] * (<W[co], dWu[co]> - mean[co] * bsum[co]);  dbeta[co] += bsum[co]
@@ -333,10 +367,11 @@ __global__ void __launch_bounds__(kThreads) head_fwd_kernel(const float4* __rest
   }
 }
 
+template <bool ORD = false>
 __global__ void __launch_bounds__(kThreads) head_bwd_kernel(const float4* __restrict__ x, const float* __restrict__ w,
                                                             const float* __restrict__ b, const float* __restrict__ gd,
                                                             float4* __restrict__ gx, float* __restrict__ gw, float* __restrict__ gb, long P,
-                                                            int relu_mask, int round_out) {
+                                                            int relu_mask, int round_out, float* __restrict__ ord) {
   DVD_PDL_ENTER();
   __shared__ float ws[32];
   __shared__ float red[kThreads / 32][33];
@@ -384,7 +419,8 @@ __global__ void __launch_bounds__(kThreads) head_bwd_kernel(const float4* __rest
   if (threadIdx.x < 33) {
     float s = 0.f;
     for (int k = 0; k < kThreads / 32; ++k) s += red[k][threadIdx.x];
-    atomicAdd(threadIdx.x < 32 ? gw + threadIdx.x : gb, s);
+    if constexpr (ORD) ord[(size_t)blockIdx.x * 33 + threadIdx.x] = s;     // ordered variant: added in CTA order by ordered_sum
+    else atomicAdd(threadIdx.x < 32 ? gw + threadIdx.x : gb, s);
   }
 }
 
@@ -400,8 +436,8 @@ extern "C" int dvd_round_tf32(const float* x, float* y, long n, void* stream) {
   return 0;
 }
 
-extern "C" int dvd_relu_bwd_colsum(const float* g, const float* y, float* gm, float* colsum, const float* bn_mean, const float* bn_var,
-                                   float bn_eps, float* dgamma, long P, int C, int round_out, void* stream) {
+static int relu_bwd_colsum(const float* g, const float* y, float* gm, float* colsum, const float* bn_mean, const float* bn_var,
+                           float bn_eps, float* dgamma, long P, int C, int round_out, void* ws, size_t ws_bytes, void* stream) {
   DVD_ARG_CHECK(g && P > 0 && C > 0 && C % 4 == 0, "bad arguments (C must be a multiple of 4)");
   DVD_ARG_CHECK(!dgamma || (bn_mean && bn_var), "dgamma needs the BatchNorm statistics");
   DVD_ARG_CHECK(aligned16(g) && (!y || aligned16(y)) && (!gm || aligned16(gm)), "buffers must be 16-byte aligned");
@@ -415,10 +451,33 @@ extern "C" int dvd_relu_bwd_colsum(const float* g, const float* y, float* gm, fl
   if (gx_blocks > cap) gx_blocks = cap;
   if (gx_blocks < 1) gx_blocks = 1;
   dim3 grid((unsigned)gx_blocks, (unsigned)((c4 + cgb - 1) / cgb));
-  dvd::launch(relu_bwd_colsum_kernel, grid, kThreads, 0, (cudaStream_t)stream, (const float4*)g, (const float4*)y, (float4*)gm, colsum, bn_mean,
-                                                                    bn_var, bn_eps, dgamma, P, c4, cgb, round_out);
+  if (ws && (colsum || dgamma)) {
+    DVD_ARG_CHECK(aligned16(ws) && (size_t)gx_blocks * C * sizeof(float) <= ws_bytes,
+                  "ordered column sums: the workspace needs dvd_ordered_workspace_bytes(DVD_ORD_CHANNEL_SUMS) bytes (C <= %d)",
+                  DVD_ORD_MAX_CHANNELS);
+    dvd::launch(relu_bwd_colsum_kernel<true>, grid, kThreads, 0, (cudaStream_t)stream, (const float4*)g, (const float4*)y, (float4*)gm,
+                colsum, bn_mean, bn_var, bn_eps, dgamma, P, c4, cgb, round_out, (float*)ws);
+    DVD_CUDA_LAUNCH_CHECK("relu_bwd_colsum_kernel<ordered>");
+    dvd::launch(colsum_ordered_reduce_kernel, (unsigned)((C + kThreads - 1) / kThreads), kThreads, 0, (cudaStream_t)stream,
+                (const float*)ws, (int)gx_blocks, C, colsum, bn_mean, bn_var, bn_eps, dgamma);
+    DVD_CUDA_LAUNCH_CHECK("colsum_ordered_reduce_kernel");
+    return 0;
+  }
+  dvd::launch(relu_bwd_colsum_kernel<>, grid, kThreads, 0, (cudaStream_t)stream, (const float4*)g, (const float4*)y, (float4*)gm, colsum, bn_mean,
+                                                                    bn_var, bn_eps, dgamma, P, c4, cgb, round_out, (float*)nullptr);
   DVD_CUDA_LAUNCH_CHECK("relu_bwd_colsum_kernel");
   return 0;
+}
+
+extern "C" int dvd_relu_bwd_colsum(const float* g, const float* y, float* gm, float* colsum, const float* bn_mean, const float* bn_var,
+                                   float bn_eps, float* dgamma, long P, int C, int round_out, void* stream) {
+  return relu_bwd_colsum(g, y, gm, colsum, bn_mean, bn_var, bn_eps, dgamma, P, C, round_out, nullptr, 0, stream);
+}
+extern "C" int dvd_relu_bwd_colsum_ordered(const float* g, const float* y, float* gm, float* colsum, const float* bn_mean,
+                                           const float* bn_var, float bn_eps, float* dgamma, long P, int C, int round_out, void* ws,
+                                           size_t ws_bytes, void* stream) {
+  DVD_ARG_CHECK(ws != nullptr, "dvd_relu_bwd_colsum_ordered: null workspace");
+  return relu_bwd_colsum(g, y, gm, colsum, bn_mean, bn_var, bn_eps, dgamma, P, C, round_out, ws, ws_bytes, stream);
 }
 
 extern "C" int dvd_maxpool3x3s2_fwd(const float* x, float* y, unsigned char* idx, int N, int H, int W, int C, void* stream) {
@@ -459,10 +518,10 @@ extern "C" int dvd_stem_fwd(const float* x_nchw, const float* weight, long s_co,
   return 0;
 }
 
-extern "C" int dvd_stem_wgrad(const float* x_nchw, const float* g, const float* a0, const float* weight, float* dweight, long s_co,
-                              long s_ci, long s_ky, long s_kx, const float* bn_gamma, const float* bn_mean, const float* bn_var,
-                              float bn_eps, float* dgamma, float* dbeta, const float* norm_mean3, const float* norm_std3, float* scratch,
-                              int N, int H, int W, void* stream) {
+static int stem_wgrad(const float* x_nchw, const float* g, const float* a0, const float* weight, float* dweight, long s_co,
+                      long s_ci, long s_ky, long s_kx, const float* bn_gamma, const float* bn_mean, const float* bn_var,
+                      float bn_eps, float* dgamma, float* dbeta, const float* norm_mean3, const float* norm_std3, float* scratch,
+                      int N, int H, int W, void* ws, size_t ws_bytes, void* stream) {
   DVD_ARG_CHECK(x_nchw && g && a0 && weight && dweight && bn_gamma && bn_mean && bn_var && dgamma && dbeta && scratch, "null pointer");
   DVD_ARG_CHECK(N > 0 && H > 0 && W > 0, "bad shape");
   const int OH = (H + 6 - 7) / 2 + 1, OW = (W + 6 - 7) / 2 + 1;
@@ -473,12 +532,40 @@ extern "C" int dvd_stem_wgrad(const float* x_nchw, const float* g, const float* 
   const int ntiles = N * ((OH + kStemTH - 1) / kStemTH) * ((OW + kStemTW - 1) / kStemTW);
   int grid = num_sms() * 2;
   if (grid > ntiles) grid = ntiles;
-  dvd::launch(stem_wgrad_kernel, grid, 256, 0, (cudaStream_t)stream, x_nchw, g, a0, nm, nr, scratch, scratch + kStemTaps * 64, N, H, W, OH, OW);
-  DVD_CUDA_LAUNCH_CHECK("stem_wgrad_kernel");
+  if (ws) {
+    constexpr int kSlab = kStemTaps * 64 + 64;
+    DVD_ARG_CHECK(aligned16(ws) && (size_t)grid * kSlab * sizeof(float) <= ws_bytes,
+                  "ordered stem weight gradient: the workspace needs dvd_ordered_workspace_bytes(DVD_ORD_STEM) bytes");
+    dvd::launch(stem_wgrad_kernel<true>, grid, 256, 0, (cudaStream_t)stream, x_nchw, g, a0, nm, nr, scratch, scratch + kStemTaps * 64, N,
+                H, W, OH, OW, (float*)ws);
+    DVD_CUDA_LAUNCH_CHECK("stem_wgrad_kernel<ordered>");
+    if (int e = launch_ordered_sum((const float*)ws, grid, kSlab, scratch, kSlab, nullptr, (cudaStream_t)stream)) return e;
+  } else {
+    dvd::launch(stem_wgrad_kernel<>, grid, 256, 0, (cudaStream_t)stream, x_nchw, g, a0, nm, nr, scratch, scratch + kStemTaps * 64, N, H, W,
+                OH, OW, (float*)nullptr);
+    DVD_CUDA_LAUNCH_CHECK("stem_wgrad_kernel");
+  }
   dvd::launch(stem_wgrad_finalize_kernel, 1, 64, 0, (cudaStream_t)stream, scratch, scratch + kStemTaps * 64, weight, dweight, s_co, s_ci, s_ky, s_kx,
                                                                 bn_gamma, bn_mean, bn_var, bn_eps, dgamma, dbeta);
   DVD_CUDA_LAUNCH_CHECK("stem_wgrad_finalize_kernel");
   return 0;
+}
+
+extern "C" int dvd_stem_wgrad(const float* x_nchw, const float* g, const float* a0, const float* weight, float* dweight, long s_co,
+                              long s_ci, long s_ky, long s_kx, const float* bn_gamma, const float* bn_mean, const float* bn_var,
+                              float bn_eps, float* dgamma, float* dbeta, const float* norm_mean3, const float* norm_std3, float* scratch,
+                              int N, int H, int W, void* stream) {
+  return stem_wgrad(x_nchw, g, a0, weight, dweight, s_co, s_ci, s_ky, s_kx, bn_gamma, bn_mean, bn_var, bn_eps, dgamma, dbeta, norm_mean3,
+                    norm_std3, scratch, N, H, W, nullptr, 0, stream);
+}
+extern "C" int dvd_stem_wgrad_ordered(const float* x_nchw, const float* g, const float* a0, const float* weight, float* dweight,
+                                      long s_co, long s_ci, long s_ky, long s_kx, const float* bn_gamma, const float* bn_mean,
+                                      const float* bn_var, float bn_eps, float* dgamma, float* dbeta, const float* norm_mean3,
+                                      const float* norm_std3, float* scratch, int N, int H, int W, void* ws, size_t ws_bytes,
+                                      void* stream) {
+  DVD_ARG_CHECK(ws != nullptr, "dvd_stem_wgrad_ordered: null workspace");
+  return stem_wgrad(x_nchw, g, a0, weight, dweight, s_co, s_ci, s_ky, s_kx, bn_gamma, bn_mean, bn_var, bn_eps, dgamma, dbeta, norm_mean3,
+                    norm_std3, scratch, N, H, W, ws, ws_bytes, stream);
 }
 
 extern "C" int dvd_head_fwd(const float* x, const float* w, const float* b, float* depth, long P, void* stream) {
@@ -488,10 +575,30 @@ extern "C" int dvd_head_fwd(const float* x, const float* w, const float* b, floa
   return 0;
 }
 
-extern "C" int dvd_head_bwd(const float* x, const float* w, const float* b, const float* g_depth, float* gx, float* gw, float* gb, long P,
-                            int relu_mask, int round_out, void* stream) {
+static int head_bwd(const float* x, const float* w, const float* b, const float* g_depth, float* gx, float* gw, float* gb, long P,
+                    int relu_mask, int round_out, void* ws, size_t ws_bytes, void* stream) {
   DVD_ARG_CHECK(x && w && b && g_depth && gx && gw && gb && P > 0 && aligned16(x) && aligned16(gx), "bad arguments");
-  dvd::launch(head_bwd_kernel, blocks_for(P, 4), kThreads, 0, (cudaStream_t)stream, (const float4*)x, w, b, g_depth, (float4*)gx, gw, gb, P, relu_mask, round_out);
+  if (ws) {
+    const unsigned grid = blocks_for(P, 4);
+    DVD_ARG_CHECK(aligned16(ws) && (size_t)grid * 33 * sizeof(float) <= ws_bytes,
+                  "ordered head gradient: the workspace needs dvd_ordered_workspace_bytes(DVD_ORD_HEAD) bytes");
+    dvd::launch(head_bwd_kernel<true>, grid, kThreads, 0, (cudaStream_t)stream, (const float4*)x, w, b, g_depth, (float4*)gx, gw, gb, P,
+                relu_mask, round_out, (float*)ws);
+    DVD_CUDA_LAUNCH_CHECK("head_bwd_kernel<ordered>");
+    return launch_ordered_sum((const float*)ws, (int)grid, 33, gw, 32, gb, (cudaStream_t)stream);
+  }
+  dvd::launch(head_bwd_kernel<>, blocks_for(P, 4), kThreads, 0, (cudaStream_t)stream, (const float4*)x, w, b, g_depth, (float4*)gx, gw, gb, P, relu_mask, round_out,
+              (float*)nullptr);
   DVD_CUDA_LAUNCH_CHECK("head_bwd_kernel");
   return 0;
+}
+
+extern "C" int dvd_head_bwd(const float* x, const float* w, const float* b, const float* g_depth, float* gx, float* gw, float* gb, long P,
+                            int relu_mask, int round_out, void* stream) {
+  return head_bwd(x, w, b, g_depth, gx, gw, gb, P, relu_mask, round_out, nullptr, 0, stream);
+}
+extern "C" int dvd_head_bwd_ordered(const float* x, const float* w, const float* b, const float* g_depth, float* gx, float* gw,
+                                    float* gb, long P, int relu_mask, int round_out, void* ws, size_t ws_bytes, void* stream) {
+  DVD_ARG_CHECK(ws != nullptr, "dvd_head_bwd_ordered: null workspace");
+  return head_bwd(x, w, b, g_depth, gx, gw, gb, P, relu_mask, round_out, ws, ws_bytes, stream);
 }

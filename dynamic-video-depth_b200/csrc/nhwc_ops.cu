@@ -53,12 +53,13 @@ __global__ void __launch_bounds__(kElemThreads) bn_act_fwd_kernel(const float4* 
 // backward of the above: gm = g * [y > 0] (if relu); g_x = gm * scale; g_res = gm (optional);
 // g_gamma[c] += sum gm * (x - mean) * rstd ; g_beta[c] += sum gm.
 // block = (cgb channel-groups of 4) x (256 / cgb pixel rows); grid.x over pixel slabs, grid.y over channel blocks.
+template <bool ORD = false>
 __global__ void __launch_bounds__(kElemThreads) bn_act_bwd_kernel(const float4* __restrict__ g, const float4* __restrict__ x,
                                                                   const float4* __restrict__ y, const float* __restrict__ gamma,
                                                                   const float* __restrict__ mean, const float* __restrict__ var,
                                                                   float eps, float4* __restrict__ gx, float4* __restrict__ gres,
                                                                   float* __restrict__ ggamma, float* __restrict__ gbeta, long P,
-                                                                  int c4, int cgb, int relu) {
+                                                                  int c4, int cgb, int relu, float* __restrict__ ord) {
   DVD_PDL_ENTER();
   __shared__ float red[kElemThreads][8];
   const int tx = threadIdx.x % cgb, ty = threadIdx.x / cgb, rows = kElemThreads / cgb;
@@ -98,10 +99,16 @@ __global__ void __launch_bounds__(kElemThreads) bn_act_bwd_kernel(const float4* 
     for (int r = 0; r < rows; ++r)
 #pragma unroll
       for (int k = 0; k < 8; ++k) a[k] += red[r * cgb + tx][k];
+    if constexpr (ORD) {   // ordered variant: [CTA column][gamma C | beta C] slab, added in CTA order by ordered_sum
+      float* o = ord + (size_t)blockIdx.x * 8 * c4 + cg * 4;
+#pragma unroll
+      for (int k = 0; k < 4; ++k) { o[k] = a[k]; o[4 * c4 + k] = a[4 + k]; }
+    } else {
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       atomicAdd(ggamma + cg * 4 + k, a[k]);
       atomicAdd(gbeta + cg * 4 + k, a[4 + k]);
+    }
     }
   }
 }
@@ -215,9 +222,9 @@ extern "C" int dvd_bn_act_fwd(const float* x, const float* res, const float* gam
   return 0;
 }
 
-extern "C" int dvd_bn_act_bwd(const float* g, const float* x, const float* y, const float* gamma, const float* mean,
-                              const float* var, float eps, float* gx, float* gres, float* ggamma, float* gbeta, long P, int C,
-                              int relu, void* stream) {
+static int bn_act_bwd(const float* g, const float* x, const float* y, const float* gamma, const float* mean,
+                      const float* var, float eps, float* gx, float* gres, float* ggamma, float* gbeta, long P, int C,
+                      int relu, void* ws, size_t ws_bytes, void* stream) {
   DVD_ARG_CHECK(g && x && gamma && mean && var && gx && ggamma && gbeta, "null pointer");
   DVD_ARG_CHECK(!relu || y, "y is required for the ReLU mask");
   DVD_ARG_CHECK(P > 0 && C > 0 && C % 4 == 0, "C must be a positive multiple of 4 (got %d)", C);
@@ -231,11 +238,32 @@ extern "C" int dvd_bn_act_bwd(const float* g, const float* x, const float* y, co
   if (gx_blocks > cap) gx_blocks = cap;
   if (gx_blocks < 1) gx_blocks = 1;
   dim3 grid((unsigned)gx_blocks, (unsigned)((c4 + cgb - 1) / cgb));
-  dvd::launch(bn_act_bwd_kernel, grid, kElemThreads, 0, (cudaStream_t)stream, (const float4*)g, (const float4*)x, (const float4*)y, gamma, mean,
+  if (ws) {
+    DVD_ARG_CHECK(aligned16(ws) && (size_t)gx_blocks * 2 * C * sizeof(float) <= ws_bytes,
+                  "ordered BatchNorm gradient: the workspace needs dvd_ordered_workspace_bytes(DVD_ORD_CHANNEL_SUMS) bytes (C <= %d)",
+                  DVD_ORD_MAX_CHANNELS);
+    dvd::launch(bn_act_bwd_kernel<true>, grid, kElemThreads, 0, (cudaStream_t)stream, (const float4*)g, (const float4*)x, (const float4*)y,
+                gamma, mean, var, eps, (float4*)gx, (float4*)gres, ggamma, gbeta, P, c4, cgb, relu, (float*)ws);
+    DVD_CUDA_LAUNCH_CHECK("bn_act_bwd<ordered>");
+    return launch_ordered_sum((const float*)ws, (int)gx_blocks, 2L * C, ggamma, C, gbeta, (cudaStream_t)stream);
+  }
+  dvd::launch(bn_act_bwd_kernel<>, grid, kElemThreads, 0, (cudaStream_t)stream, (const float4*)g, (const float4*)x, (const float4*)y, gamma, mean,
                                                                      var, eps, (float4*)gx, (float4*)gres, ggamma, gbeta, P, c4, cgb,
-                                                                     relu);
+                                                                     relu, (float*)nullptr);
   DVD_CUDA_LAUNCH_CHECK("bn_act_bwd");
   return 0;
+}
+
+extern "C" int dvd_bn_act_bwd(const float* g, const float* x, const float* y, const float* gamma, const float* mean,
+                              const float* var, float eps, float* gx, float* gres, float* ggamma, float* gbeta, long P, int C,
+                              int relu, void* stream) {
+  return bn_act_bwd(g, x, y, gamma, mean, var, eps, gx, gres, ggamma, gbeta, P, C, relu, nullptr, 0, stream);
+}
+extern "C" int dvd_bn_act_bwd_ordered(const float* g, const float* x, const float* y, const float* gamma, const float* mean,
+                                      const float* var, float eps, float* gx, float* gres, float* ggamma, float* gbeta, long P, int C,
+                                      int relu, void* ws, size_t ws_bytes, void* stream) {
+  DVD_ARG_CHECK(ws != nullptr, "dvd_bn_act_bwd_ordered: null workspace");
+  return bn_act_bwd(g, x, y, gamma, mean, var, eps, gx, gres, ggamma, gbeta, P, C, relu, ws, ws_bytes, stream);
 }
 
 extern "C" int dvd_upsample2x_fwd(const float* x, float* y, int N, int H, int W, int C, int align_corners, int round_out, void* stream) {

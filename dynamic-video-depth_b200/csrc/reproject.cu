@@ -15,6 +15,7 @@
 //
 // Algorithmic HBM bytes per pixel (fp32): fwd 32 (d1 4, d2 4, flow 8, mask 4, sf 12);
 // bwd 48 (the same 32 read + g_sf 12 + g_d2 4 written). See DESIGN.md for the full accounting.
+#include <cub/device/device_radix_sort.cuh>
 #include "common.cuh"
 #include <algorithm>
 #include <initializer_list>
@@ -556,11 +557,14 @@ __global__ void __launch_bounds__(kThreads, 2) reproject_loss_fwd_kernel(
   write_block_sums(sum_slots(acc), partials + (b * gridDim.x + blockIdx.x) * 4);
 }
 
+// ORD: instead of scattering, pixel i of the launch writes its four taps as (target index into g_d2, contribution) pairs
+// at [4 i, 4 i + 4) of keys / vals; a zero contribution gets the key B * HW, which sorts after every target
+template <bool ORD = false>
 __global__ void __launch_bounds__(kThreads) reproject_loss_bwd_kernel(
     const float* __restrict__ depth_1, const float* __restrict__ depth_2, const float* __restrict__ flow,
     const float* __restrict__ mask_2, const float* __restrict__ sf, dvd_loss_cfg cfg, const float* __restrict__ scalars,
     float gscale, const float* __restrict__ gscale_dev, float* __restrict__ g_sf, float* __restrict__ g_d2, int H, int W,
-    const float* __restrict__ poses) {
+    const float* __restrict__ poses, uint32_t* __restrict__ keys, float* __restrict__ vals) {
   DVD_PDL_ENTER();
   const int HW = H * W;
   const size_t b = blockIdx.y;
@@ -581,9 +585,33 @@ __global__ void __launch_bounds__(kThreads) reproject_loss_bwd_kernel(
     if (gd2img) {
       float gd[4];
       tap_grads(o, h[0], h[1], h[2], gd);
-      scatter4_atomic(gd2img + o.i00, o.sx1, o.sy1, gd);
+      if constexpr (ORD) {
+        const uint32_t base = (uint32_t)(b * HW + o.i00), none = (uint32_t)(gridDim.y * HW);
+        const uint32_t tgt[4] = {base, base + o.sx1, base + o.sy1, base + o.sy1 + o.sx1};
+        const size_t e = 4 * (b * HW + p);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          keys[e + k] = gd[k] != 0.f ? tgt[k] : none;
+          vals[e + k] = gd[k];
+        }
+      } else {
+        scatter4_atomic(gd2img + o.i00, o.sx1, o.sy1, gd);
+      }
     }
   }
+}
+
+// g_d2[key] = the contributions of one run of equal keys, summed in their (pixel, tap) order; one thread per run start
+__global__ void __launch_bounds__(kThreads) scatter_runs_kernel(const uint32_t* __restrict__ keys, const float* __restrict__ vals,
+                                                                long n, uint32_t none, float* __restrict__ g_d2) {
+  DVD_PDL_ENTER();
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t k = keys[i];
+  if (k == none || (i > 0 && keys[i - 1] == k)) return;
+  float s = 0.f;
+  for (long j = i; j < n && keys[j] == k; ++j) s += vals[j];
+  g_d2[k] = s;
 }
 
 // deterministic final reduction (fixed order, double accumulation) + loss assembly
@@ -1119,9 +1147,66 @@ extern "C" int dvd_reproject_loss_bwd(const float* depth_1, const float* depth_2
       DVD_CUDA_LAUNCH_CHECK("reproject_loss_bwd");
       return 0;
     });
-  dvd::launch(reproject_loss_bwd_kernel, grid_for(B, HW), kThreads, 0, st, depth_1, depth_2, flow_1_2, mask_2, sf, *cfg,
-              scalars, gscale, gscale_dev, g_sf, g_depth_2, H, W, poses);
+  dvd::launch(reproject_loss_bwd_kernel<>, grid_for(B, HW), kThreads, 0, st, depth_1, depth_2, flow_1_2, mask_2, sf, *cfg,
+              scalars, gscale, gscale_dev, g_sf, g_depth_2, H, W, poses, (uint32_t*)nullptr, (float*)nullptr);
   DVD_CUDA_LAUNCH_CHECK("reproject_loss_bwd");
+  return 0;
+}
+
+// workspace of the ordered backward: keys and values before and after the sort (16 B per tap), then CUB's temporary storage
+static int ordered_layout(int B, int H, int W, size_t* temp_bytes, size_t* total) {
+  const long n = 4L * B * H * W;
+  const uint32_t none = (uint32_t)((long)B * H * W);
+  const int end_bit = 32 - __builtin_clz(none);
+  *temp_bytes = 0;
+  DVD_CUDA_CALL(cub::DeviceRadixSort::SortPairs(nullptr, *temp_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr,
+                                                (const float*)nullptr, (float*)nullptr, n, 0, end_bit));
+  *total = 16 * (size_t)n + *temp_bytes + 256;
+  return 0;
+}
+
+extern "C" size_t dvd_reproject_ordered_bytes(int B, int H, int W) {
+  if (B < 1 || H < 2 || W < 2 || (long)B * H * W >= (1L << 30)) return 0;
+  size_t temp = 0, total = 0;
+  if (ordered_layout(B, H, W, &temp, &total)) return 0;
+  return total;
+}
+
+extern "C" int dvd_reproject_loss_bwd_ordered(const float* depth_1, const float* depth_2, const float* flow_1_2,
+                                              const float* mask_2, const float* sf, const float* poses,
+                                              const dvd_loss_cfg* cfg, const float* scalars, float gscale,
+                                              const float* gscale_dev, float* g_sf, float* g_depth_2, int B, int H, int W,
+                                              void* ws, size_t ws_bytes, void* stream) {
+  if (!g_depth_2)      // no scatter: the default launch is already deterministic
+    return dvd_reproject_loss_bwd(depth_1, depth_2, flow_1_2, mask_2, sf, poses, cfg, scalars, gscale, gscale_dev, g_sf, g_depth_2,
+                                  B, H, W, stream);
+  if (int e = check_shape(B, H, W)) return e;
+  if (int e = check_cfg(cfg)) return e;
+  DVD_ARG_CHECK(depth_1 && depth_2 && flow_1_2 && mask_2 && sf && poses && scalars && g_sf && ws, "null pointer");
+  DVD_ARG_CHECK((long)B * H * W < (1L << 30), "too many pixels for the ordered backward");
+  size_t temp = 0, total = 0;
+  if (int e = ordered_layout(B, H, W, &temp, &total)) return e;
+  DVD_ARG_CHECK(ws_bytes >= total && aligned16(ws), "ordered re-projection backward: the workspace needs "
+                "dvd_reproject_ordered_bytes(B, H, W) = %zu bytes, 16-byte aligned", total);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int HW = H * W;
+  const long n = 4L * B * HW;
+  const uint32_t none = (uint32_t)((long)B * HW);
+  uint32_t* k_in = (uint32_t*)ws;
+  float* v_in = (float*)(k_in + n);
+  uint32_t* k_out = (uint32_t*)(v_in + n);
+  float* v_out = (float*)(k_out + n);
+  void* temp_ptr = (void*)(((uintptr_t)(v_out + n) + 255) & ~(uintptr_t)255);
+  DVD_CUDA_CALL(cudaMemsetAsync(g_depth_2, 0, (size_t)B * HW * sizeof(float), st));
+  // the generic kernel for every shape: its per-pixel results equal the staged kernel's bit for bit
+  dvd::launch(reproject_loss_bwd_kernel<true>, grid_for(B, HW), kThreads, 0, st, depth_1, depth_2, flow_1_2, mask_2, sf, *cfg,
+              scalars, gscale, gscale_dev, g_sf, g_depth_2, H, W, poses, k_in, v_in);
+  DVD_CUDA_LAUNCH_CHECK("reproject_loss_bwd<ordered>");
+  DVD_CUDA_CALL(cub::DeviceRadixSort::SortPairs(temp_ptr, temp, (const uint32_t*)k_in, k_out, (const float*)v_in, v_out, n, 0,
+                                                32 - __builtin_clz(none), st));
+  dvd::launch(scatter_runs_kernel, (unsigned)((n + kThreads - 1) / kThreads), kThreads, 0, st, (const uint32_t*)k_out,
+              (const float*)v_out, n, none, g_depth_2);
+  DVD_CUDA_LAUNCH_CHECK("scatter_runs_kernel");
   return 0;
 }
 

@@ -442,10 +442,11 @@ struct DgradParams {
   long npx, hw;
   MlpLayout L;
   dvd_mlp_cfg cfg;
+  float* ord;      // ordered variant: [CTA][MMA warp][3] output-bias partials
 };
 
 // KPAD: the layer-0 width L.kpad0 (the N of its MMA)
-template <int FX, int FT, bool TD, int KPAD>
+template <int FX, int FT, bool TD, int KPAD, bool ORD = false>
 __global__ void __launch_bounds__(kThreadsMlp, 1) mlp_dgrad_kernel(const __grid_constant__ DgradParams P) {
   using E = Embed<FX, FT, TD>;
   static_assert(!E::kStatic || KPAD == E::KPAD, "layer-0 width of a specialised configuration");
@@ -641,10 +642,18 @@ __global__ void __launch_bounds__(kThreadsMlp, 1) mlp_dgrad_kernel(const __grid_
   save_image_wait_all();
   // output-layer bias gradient: warp reduce, one atomic per warp
   b5x = warp_sum(b5x); b5y = warp_sum(b5y); b5z = warp_sum(b5z);
+  if constexpr (ORD) {
+    // the slabs are added in (CTA, warp) order by ordered_sum
+    if (lane == 0 && P.g_bias5) {
+      float* o = P.ord + ((size_t)blockIdx.x * 8 + (warp - 4)) * 3;
+      o[0] = b5x; o[1] = b5y; o[2] = b5z;
+    }
+  } else {
   if (lane == 0 && P.g_bias5) {
     atomicAdd(P.g_bias5 + 0, b5x);
     atomicAdd(P.g_bias5 + 1, b5y);
     atomicAdd(P.g_bias5 + 2, b5z);
+  }
   }
 }
 
@@ -664,7 +673,10 @@ struct WgradJob {
 struct WgradParams {
   WgradJob job[12];
   long nq;
+  int nsplit;      // gridDim.y of the ordered variant
+  float* ord;      // ordered variant: per CTA (job, split) a slab of kOrdSlab floats: [128 rows][256 columns], then 128 bias sums
 };
+constexpr int kOrdSlab = 128 * 256 + 128;
 constexpr int kWgStages = 4;
 constexpr uint32_t kWgStageBytes = kSavePlanes * (16384 + 32768);      // per plane: A 128 ch x 64 px, B up to 256 ch x 64 px (bf16)
 constexpr size_t kWgradSmemBytes = 1024 + (size_t)kWgStages * kWgStageBytes + 8192 + 256;
@@ -684,9 +696,9 @@ __device__ __forceinline__ void wgrad_mma(float (&acc)[N / 2], float (&accb)[8],
   fence_regs(accb);
 }
 
-template <int N>
+template <int N, bool ORD>
 __device__ __forceinline__ void wgrad_consume(const WgradJob& J, uint8_t* const* stage, uint64_t* full, uint64_t* empty, uint32_t so,
-                                              long q0, long q1) {
+                                              long q0, long q1, float* slab) {
   const int wg = threadIdx.x >> 7, cw = wg - 1, warp = threadIdx.x >> 5, lane = threadIdx.x & 31, t4 = lane & 3;
   float acc[N / 2], accb[8];
 #pragma unroll
@@ -702,6 +714,22 @@ __device__ __forceinline__ void wgrad_consume(const WgradJob& J, uint8_t* const*
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[s]);
   }
+  if constexpr (ORD) {
+    // this CTA's slab; mlp_wgrad_reduce_kernel adds the slabs of a job in split order
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int ml = cw * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+      if (J.m_off + ml >= J.m_valid) continue;
+#pragma unroll
+      for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const int n = 8 * j + 2 * t4 + c;
+          if (n < J.n_valid) slab[ml * 256 + n] = acc[4 * j + 2 * h + c];
+        }
+      if (J.bias_out && t4 == 0) slab[128 * 256 + ml] = accb[2 * h];
+    }
+  } else {
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int m = J.m_off + cw * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
@@ -718,8 +746,10 @@ __device__ __forceinline__ void wgrad_consume(const WgradJob& J, uint8_t* const*
       }
     if (J.bias_out && t4 == 0) atomicAdd(J.bias_out + m, accb[2 * h]);
   }
+  }
 }
 
+template <bool ORD = false>
 __global__ void __launch_bounds__(kThreadsWgrad, 1) mlp_wgrad_kernel(const __grid_constant__ WgradParams P) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -762,15 +792,37 @@ __global__ void __launch_bounds__(kThreadsWgrad, 1) mlp_wgrad_kernel(const __gri
   }
   if (q1 <= q0) return;
   const uint32_t so = smem_u32(ones);
+  float* slab = ORD ? P.ord + ((size_t)blockIdx.x * gridDim.y + blockIdx.y) * kOrdSlab : nullptr;
   switch (J.n) {
-    case 256: wgrad_consume<256>(J, stage, full, empty, so, q0, q1); break;
-    case 192: wgrad_consume<192>(J, stage, full, empty, so, q0, q1); break;
-    case 144: wgrad_consume<144>(J, stage, full, empty, so, q0, q1); break;
-    case 128: wgrad_consume<128>(J, stage, full, empty, so, q0, q1); break;
-    case 112: wgrad_consume<112>(J, stage, full, empty, so, q0, q1); break;
-    case 64: wgrad_consume<64>(J, stage, full, empty, so, q0, q1); break;
-    case 16: wgrad_consume<16>(J, stage, full, empty, so, q0, q1); break;
+    case 256: wgrad_consume<256, ORD>(J, stage, full, empty, so, q0, q1, slab); break;
+    case 192: wgrad_consume<192, ORD>(J, stage, full, empty, so, q0, q1, slab); break;
+    case 144: wgrad_consume<144, ORD>(J, stage, full, empty, so, q0, q1, slab); break;
+    case 128: wgrad_consume<128, ORD>(J, stage, full, empty, so, q0, q1, slab); break;
+    case 112: wgrad_consume<112, ORD>(J, stage, full, empty, so, q0, q1, slab); break;
+    case 64: wgrad_consume<64, ORD>(J, stage, full, empty, so, q0, q1, slab); break;
+    case 16: wgrad_consume<16, ORD>(J, stage, full, empty, so, q0, q1, slab); break;
     default: __trap();   // dvd_mlp_wgrad only builds jobs of these widths (checked there as well)
+  }
+}
+
+// out[m, n] (or out[n, m]) += the job's split partials in split order; bias_out[m] likewise. blockIdx.x = job, blockIdx.y =
+// row of the job's 128, thread = column; nparts: the splits with a non-empty pixel range
+__global__ void __launch_bounds__(256) mlp_wgrad_reduce_kernel(const __grid_constant__ WgradParams P, int nparts) {
+  DVD_PDL_ENTER();
+  const WgradJob& J = P.job[blockIdx.x];
+  const int ml = blockIdx.y, m = J.m_off + ml, n = threadIdx.x;
+  if (m >= J.m_valid) return;
+  const float* src = P.ord + (size_t)blockIdx.x * P.nsplit * kOrdSlab;
+  if (n < J.n_valid) {
+    float s = 0.f;
+    for (int p = 0; p < nparts; ++p) s += __ldcg(src + (size_t)p * kOrdSlab + ml * 256 + n);
+    float* dst = J.transposed ? J.out + (size_t)n * J.ld + m : J.out + (size_t)m * J.ld + n;
+    *dst += s;
+  }
+  if (J.bias_out && n == 0) {
+    float s = 0.f;
+    for (int p = 0; p < nparts; ++p) s += __ldcg(src + (size_t)p * kOrdSlab + 128 * 256 + ml);
+    J.bias_out[m] += s;
   }
 }
 
@@ -910,6 +962,14 @@ extern "C" int dvd_mlp_chain_fwd(const dvd_mlp_cfg* cfg, const void* packed_fwd,
 
 template <int FX, int FT, bool TD, int KPAD>
 static int launch_dgrad(const DgradParams& P, cudaStream_t st) {
+  if (P.ord) {
+    const int grid = chain_grid(P.L.ntiles);
+    DVD_CUDA_CALL(cudaFuncSetAttribute(mlp_dgrad_kernel<FX, FT, TD, KPAD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)kChainSmemBytes));
+    dvd::launch(mlp_dgrad_kernel<FX, FT, TD, KPAD, true>, grid, kThreadsMlp, kChainSmemBytes, st, P);
+    DVD_CUDA_LAUNCH_CHECK("mlp_dgrad<ordered>");
+    return P.g_bias5 ? launch_ordered_sum(P.ord, grid * 8, 3, P.g_bias5, 3, nullptr, st) : 0;
+  }
   DVD_CUDA_CALL(cudaFuncSetAttribute(mlp_dgrad_kernel<FX, FT, TD, KPAD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)kChainSmemBytes));
   dvd::launch(mlp_dgrad_kernel<FX, FT, TD, KPAD>, chain_grid(P.L.ntiles), kThreadsMlp, kChainSmemBytes, st, P);
@@ -917,10 +977,10 @@ static int launch_dgrad(const DgradParams& P, cudaStream_t st) {
   return 0;
 }
 
-extern "C" int dvd_mlp_dgrad(const dvd_mlp_cfg* cfg, const void* packed_bwd, const float* p_e, const float* t0, float dt,
-                             int e, int use_g_acc, const float* g_acc, const float* g_step, const float* a_in,
-                             float* a_out, const void* save_e, void* dy_scratch, float* g_bias5, long npx, long hw,
-                             void* stream) {
+static int mlp_dgrad(const dvd_mlp_cfg* cfg, const void* packed_bwd, const float* p_e, const float* t0, float dt,
+                     int e, int use_g_acc, const float* g_acc, const float* g_step, const float* a_in,
+                     float* a_out, const void* save_e, void* dy_scratch, float* g_bias5, long npx, long hw,
+                     void* ws, size_t ws_bytes, void* stream) {
   int variant;
   if (int er = check_cfg_supported(cfg, &variant)) return er;
   DVD_ARG_CHECK(packed_bwd && p_e && save_e && dy_scratch, "null pointer");
@@ -931,6 +991,9 @@ extern "C" int dvd_mlp_dgrad(const dvd_mlp_cfg* cfg, const void* packed_bwd, con
   P.wb = (const uint8_t*)packed_bwd; P.p_e = p_e; P.t0 = t0; P.dt = dt; P.e = e; P.use_g_acc = use_g_acc;
   P.g_acc = g_acc; P.g_step = g_step; P.a_in = a_in; P.a_out = a_out; P.save_e = (const uint8_t*)save_e;
   P.dy = (uint8_t*)dy_scratch; P.g_bias5 = g_bias5; P.npx = npx; P.hw = hw; P.L = make_layout(*cfg, npx); P.cfg = *cfg;
+  P.ord = (float*)ws;
+  DVD_ARG_CHECK(!ws || ws_bytes >= (size_t)chain_grid(P.L.ntiles) * 8 * 3 * sizeof(float),
+                "ordered MLP data gradient: the workspace needs dvd_ordered_workspace_bytes(DVD_ORD_MLP_DGRAD) bytes");
   cudaStream_t st = (cudaStream_t)stream;
   if (variant == 0) return launch_dgrad<16, 16, true, Embed<16, 16, true>::KPAD>(P, st);
   if (variant == 1) return launch_dgrad<16, 0, false, Embed<16, 0, false>::KPAD>(P, st);
@@ -942,8 +1005,8 @@ extern "C" int dvd_mlp_dgrad(const dvd_mlp_cfg* cfg, const void* packed_bwd, con
   }
 }
 
-extern "C" int dvd_mlp_wgrad(const dvd_mlp_cfg* cfg, const void* save_e, const void* dy_scratch, float* const* g_w,
-                             float* const* g_b, long npx, void* stream) {
+static int mlp_wgrad(const dvd_mlp_cfg* cfg, const void* save_e, const void* dy_scratch, float* const* g_w,
+                     float* const* g_b, long npx, void* ws, size_t ws_bytes, void* stream) {
   int variant;
   if (int er = check_cfg_supported(cfg, &variant)) return er;
   DVD_ARG_CHECK(save_e && dy_scratch && g_w && g_b, "null pointer");
@@ -953,6 +1016,8 @@ extern "C" int dvd_mlp_wgrad(const dvd_mlp_cfg* cfg, const void* save_e, const v
   const uint8_t* dy = (const uint8_t*)dy_scratch;
   WgradParams P;
   P.nq = L.nq;
+  P.ord = nullptr;
+  P.nsplit = 0;
   int nj = 0;
   for (int l = 0; l < kLayers; ++l) {
     DVD_ARG_CHECK(g_w[l] != nullptr, "null g_w[%d]", l);
@@ -978,10 +1043,50 @@ extern "C" int dvd_mlp_wgrad(const dvd_mlp_cfg* cfg, const void* save_e, const v
   int ksplit = num_sms() / nj;
   if (ksplit < 1) ksplit = 1;
   if ((long)ksplit > L.nq) ksplit = (int)L.nq;
-  DVD_CUDA_CALL(cudaFuncSetAttribute(mlp_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kWgradSmemBytes));
-  dvd::launch(mlp_wgrad_kernel, dim3(nj, ksplit), kThreadsWgrad, kWgradSmemBytes, (cudaStream_t)stream, P);
+  if (ws) {
+    // ordered: the same split, partial tiles through the workspace, added in split order by mlp_wgrad_reduce_kernel
+    DVD_ARG_CHECK(ws_bytes >= (size_t)nj * ksplit * kOrdSlab * sizeof(float),
+                  "ordered MLP weight gradient: the workspace needs dvd_ordered_workspace_bytes(DVD_ORD_MLP_WGRAD) bytes");
+    P.ord = (float*)ws;
+    P.nsplit = ksplit;
+    DVD_CUDA_CALL(cudaFuncSetAttribute(mlp_wgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kWgradSmemBytes));
+    dvd::launch(mlp_wgrad_kernel<true>, dim3(nj, ksplit), kThreadsWgrad, kWgradSmemBytes, (cudaStream_t)stream, P);
+    DVD_CUDA_LAUNCH_CHECK("mlp_wgrad<ordered>");
+    const long per = (L.nq + ksplit - 1) / ksplit;
+    const int nparts = (int)((L.nq + per - 1) / per);
+    dvd::launch(mlp_wgrad_reduce_kernel, dim3(nj, 128), 256, 0, (cudaStream_t)stream, P, nparts);
+    DVD_CUDA_LAUNCH_CHECK("mlp_wgrad_reduce_kernel");
+    return 0;
+  }
+  DVD_CUDA_CALL(cudaFuncSetAttribute(mlp_wgrad_kernel<>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kWgradSmemBytes));
+  dvd::launch(mlp_wgrad_kernel<>, dim3(nj, ksplit), kThreadsWgrad, kWgradSmemBytes, (cudaStream_t)stream, P);
   DVD_CUDA_LAUNCH_CHECK("mlp_wgrad");
   return 0;
+}
+
+extern "C" int dvd_mlp_dgrad(const dvd_mlp_cfg* cfg, const void* packed_bwd, const float* p_e, const float* t0, float dt,
+                             int e, int use_g_acc, const float* g_acc, const float* g_step, const float* a_in,
+                             float* a_out, const void* save_e, void* dy_scratch, float* g_bias5, long npx, long hw,
+                             void* stream) {
+  return mlp_dgrad(cfg, packed_bwd, p_e, t0, dt, e, use_g_acc, g_acc, g_step, a_in, a_out, save_e, dy_scratch, g_bias5, npx, hw,
+                   nullptr, 0, stream);
+}
+extern "C" int dvd_mlp_dgrad_ordered(const dvd_mlp_cfg* cfg, const void* packed_bwd, const float* p_e, const float* t0,
+                                     float dt, int e, int use_g_acc, const float* g_acc, const float* g_step,
+                                     const float* a_in, float* a_out, const void* save_e, void* dy_scratch,
+                                     float* g_bias5, long npx, long hw, void* ws, size_t ws_bytes, void* stream) {
+  DVD_ARG_CHECK(ws != nullptr, "dvd_mlp_dgrad_ordered: null workspace");
+  return mlp_dgrad(cfg, packed_bwd, p_e, t0, dt, e, use_g_acc, g_acc, g_step, a_in, a_out, save_e, dy_scratch, g_bias5, npx, hw,
+                   ws, ws_bytes, stream);
+}
+extern "C" int dvd_mlp_wgrad(const dvd_mlp_cfg* cfg, const void* save_e, const void* dy_scratch, float* const* g_w,
+                             float* const* g_b, long npx, void* stream) {
+  return mlp_wgrad(cfg, save_e, dy_scratch, g_w, g_b, npx, nullptr, 0, stream);
+}
+extern "C" int dvd_mlp_wgrad_ordered(const dvd_mlp_cfg* cfg, const void* save_e, const void* dy_scratch, float* const* g_w,
+                                     float* const* g_b, long npx, void* ws, size_t ws_bytes, void* stream) {
+  DVD_ARG_CHECK(ws != nullptr, "dvd_mlp_wgrad_ordered: null workspace");
+  return mlp_wgrad(cfg, save_e, dy_scratch, g_w, g_b, npx, ws, ws_bytes, stream);
 }
 
 extern "C" int dvd_acc_reg(const float* s0, const float* s1, float acc_mul, float gscale, float* g_s0, float* g_s1,

@@ -213,7 +213,13 @@ class Model(NetInterface):
     def _step_body(self, inp, steps, dt):
         """Everything of one step that runs on the device, with NO host synchronisation (so it can be captured in a CUDA
         graph): forward, losses, ONE backward, gradient exchange, both Adam updates. `inp` = namespace of device tensors.
-        Returns (logs [9] on the device: flow, disp, sf, loss, mask-sum, cf, cd, -, acc_reg; d1, d2, sf, poses for visualisation)."""
+        Returns (logs [9] on the device: flow, disp, sf, loss, mask-sum, cf, cd, -, acc_reg; d1, d2, sf, poses for visualisation).
+        Under torch.use_deterministic_algorithms(True), read once here, every backward launch of the step takes its ordered
+        variant (DESIGN.md 2.11)."""
+        with ops.ordered_reductions(torch.are_deterministic_algorithms_enabled()):
+            return self._step_launches(inp, steps, dt)
+
+    def _step_launches(self, inp, steps, dt):
         o = self.opt
         for opt_ in self._optimizers:
             opt_.materialize().zero_grad()
@@ -334,9 +340,14 @@ class Model(NetInterface):
         return (getattr(self.opt, 'cuda_graph', True) and (self._world == 1 or getattr(self.opt, 'cuda_graph_dist', True))
                 and self.device.type == 'cuda' and self.opt.midas and not getattr(self, '_graph_broken', False))
 
+    def _graph_sig(self, b, steps, dt):
+        sig = (b['img_1'].shape[0], tuple(b['img_1'].shape[-2:]), steps, bool(self.warm), round(float(dt), 9))
+        if torch.are_deterministic_algorithms_enabled():
+            sig += ('ordered',)    # a graph captured with ordered reductions never replays without them, and vice versa
+        return sig
+
     def _graph_step(self, b, steps, dt):
-        B = b['img_1'].shape[0]
-        sig = (B, tuple(b['img_1'].shape[-2:]), steps, bool(self.warm), round(float(dt), 9))
+        sig = self._graph_sig(b, steps, dt)
         if not hasattr(self, '_graphs'):
             self._graphs, self._graph_pool, self.graph_stats = {}, None, {'captured': 0, 'replayed': 0, 'eager': 0}
         ent = self._graphs.setdefault(sig, {'seen': 0, 'graph': None})

@@ -4,6 +4,7 @@ PyTorch is plumbing here (device memory, streams, autograd graph); all arithmeti
 happens inside libdvd_b200.so. Argument / shape / dtype / contiguity violations raise ValueError
 before any launch; a non-zero return from the library raises RuntimeError (SURVEY.md §8(b)).
 """
+import contextlib
 import ctypes
 import os
 
@@ -23,6 +24,49 @@ def _stream():
 
 def _ptr(t):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else ctypes.c_void_p(0)
+
+
+# ---- ordered reductions -------------------------------------------------------------------------------------------------------
+# Under torch.use_deterministic_algorithms(True) every backward launch that would add partial sums with fp32 atomics calls its
+# *_ordered entry point instead (DESIGN.md 2.11): same split, partials through a workspace, added in a fixed order. A training
+# step reads torch's switch once and runs inside `ordered_reductions(flag)`; a launch outside a step reads the switch itself.
+_ORDERED = [None]
+
+
+@contextlib.contextmanager
+def ordered_reductions(flag):
+    prev = _ORDERED[0]
+    _ORDERED[0] = bool(flag)
+    try:
+        yield
+    finally:
+        _ORDERED[0] = prev
+
+
+def ordered():
+    """Whether the backward launches issued now take their ordered (run-to-run reproducible) variants."""
+    return torch.are_deterministic_algorithms_enabled() if _ORDERED[0] is None else _ORDERED[0]
+
+
+_ORD_WS = {}     # (device index, site) -> workspace of dvd_ordered_workspace_bytes(site) bytes
+
+
+def ordered_workspace(device, site):
+    """The workspace of one ordered-reduction site on this device (sites are separate so that launches on different streams
+    never share one). Allocated once, outside graph capture: the eager steps before a capture allocate it."""
+    idx = device.index if device.index is not None else torch.cuda.current_device()
+    ws = _ORD_WS.get((idx, site))
+    if ws is None:
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError('ordered-reduction workspace %d is allocated by an eager launch before a graph capture' % site)
+        n = _lib.load().dvd_ordered_workspace_bytes(site)
+        ws = _ORD_WS[(idx, site)] = torch.empty((n + 15) // 16 * 4, dtype=torch.float32, device=torch.device('cuda', idx))
+    return ws
+
+
+def _ws(t):
+    """(pointer, bytes) of a workspace tensor"""
+    return _ptr(t), t.numel() * t.element_size()
 
 
 def _chk(t, name, shape=None):
@@ -129,6 +173,15 @@ def reproject_loss_bwd(depth_1, depth_2, flow, mask, sf, poses, cfg, scalars, gs
     g_sf = torch.empty_like(sf)
     g_d2 = torch.empty_like(depth_2) if need_depth_grad else None
     lib = _lib.load()
+    if g_d2 is not None and ordered():
+        # the sort buffers of the ordered scatter are per call, like the step's other intermediates
+        ws = torch.empty(lib.dvd_reproject_ordered_bytes(B, H, W), dtype=torch.uint8, device=depth_1.device)
+        LAUNCHES['n'] += 3
+        _lib.check(lib.dvd_reproject_loss_bwd_ordered(_ptr(depth_1), _ptr(depth_2), _ptr(flow), _ptr(mask), _ptr(sf), _ptr(poses),
+                                                      ctypes.byref(cfg), _ptr(scalars), float(gscale), _ptr(gscale_dev),
+                                                      _ptr(g_sf), _ptr(g_d2), B, H, W, *_ws(ws), _stream()),
+                   'dvd_reproject_loss_bwd_ordered')
+        return g_sf, g_d2
     LAUNCHES['n'] += 1
     _lib.check(lib.dvd_reproject_loss_bwd(_ptr(depth_1), _ptr(depth_2), _ptr(flow), _ptr(mask), _ptr(sf), _ptr(poses),
                                           ctypes.byref(cfg), _ptr(scalars), float(gscale), _ptr(gscale_dev),
@@ -346,6 +399,18 @@ def mlp_chain_bwd(packed, fwd, t0, dt, n_acc, g_acc, g_steps, grad_w, grad_b):
     if gb5.numel() != 3:
         raise ValueError('grad of the output bias must have 3 elements')
     gw_arr, gb_arr = _ptr_array(grad_w), _ptr_array(grad_b)
+    if ordered():
+        ws_d, ws_w = _ws(ordered_workspace(dev, _lib.DVD_ORD_MLP_DGRAD)), _ws(ordered_workspace(dev, _lib.DVD_ORD_MLP_WGRAD))
+
+        def dgrad(*a):
+            LAUNCHES['n'] += 1
+            return lib.dvd_mlp_dgrad_ordered(*a[:-1], *ws_d, a[-1])
+
+        def wgrad(*a):
+            LAUNCHES['n'] += 1
+            return lib.dvd_mlp_wgrad_ordered(*a[:-1], *ws_w, a[-1])
+    else:
+        dgrad, wgrad = lib.dvd_mlp_dgrad, lib.dvd_mlp_wgrad
     for i, e in enumerate(range(n_eval - 1, -1, -1)):
         dy = dys[i % nbuf]
         if wdone[i % nbuf] is not None:
@@ -354,7 +419,7 @@ def mlp_chain_bwd(packed, fwd, t0, dt, n_acc, g_acc, g_steps, grad_w, grad_b):
         gs = g_steps[e] if g_steps is not None else None
         save_e = ctypes.c_void_p(sv.data_ptr() + e * per)
         LAUNCHES['n'] += 1
-        _lib.check(lib.dvd_mlp_dgrad(ctypes.byref(cfg), _ptr(packed.bwd), _ptr(p_steps[e]),
+        _lib.check(dgrad(ctypes.byref(cfg), _ptr(packed.bwd), _ptr(p_steps[e]),
                                      _ptr(t0) if cfg.time_dependent else ctypes.c_void_p(0), float(dt), e,
                                      int(e < n_acc and g_acc is not None), _ptr(g_acc), _ptr(gs), _ptr(a), _ptr(a_out),
                                      save_e, _ptr(dy), _ptr(gb5), npx, hw, _stream()), 'dvd_mlp_dgrad')
@@ -365,11 +430,11 @@ def mlp_chain_bwd(packed, fwd, t0, dt, n_acc, g_acc, g_steps, grad_w, grad_b):
             ev.record(main)
             side.wait_event(ev)
             with torch.cuda.stream(side):
-                _lib.check(lib.dvd_mlp_wgrad(ctypes.byref(cfg), save_e, _ptr(dy), gw_arr, gb_arr, npx, _stream()), 'dvd_mlp_wgrad')
+                _lib.check(wgrad(ctypes.byref(cfg), save_e, _ptr(dy), gw_arr, gb_arr, npx, _stream()), 'dvd_mlp_wgrad')
                 wdone[i % nbuf] = torch.cuda.Event()
                 wdone[i % nbuf].record(side)
         else:
-            _lib.check(lib.dvd_mlp_wgrad(ctypes.byref(cfg), save_e, _ptr(dy), gw_arr, gb_arr, npx, _stream()), 'dvd_mlp_wgrad')
+            _lib.check(wgrad(ctypes.byref(cfg), save_e, _ptr(dy), gw_arr, gb_arr, npx, _stream()), 'dvd_mlp_wgrad')
     if side is not None:       # join: the weight gradients are final (and dY / the saved activations may be freed) after this
         for ev in wdone:
             if ev is not None:
@@ -487,9 +552,16 @@ class BnAct(torch.autograd.Function):
             ggb = torch.zeros(2, C, dtype=torch.float32, device=x.device)   # one fill for both per-channel sums
             gg, gb = ggb[0], ggb[1]
         lib = _lib.load()
-        LAUNCHES['n'] += 1
-        _lib.check(lib.dvd_bn_act_bwd(_ptr(g), _ptr(x), _ptr(y), _ptr(gamma), _ptr(mean), _ptr(var), ctx.eps, _ptr(gx), _ptr(gres),
-                                      _ptr(gg), _ptr(gb), N * H * W, C, int(ctx.relu), _stream()), 'dvd_bn_act_bwd')
+        if ordered():
+            LAUNCHES['n'] += 2
+            ws = _ws(ordered_workspace(x.device, _lib.DVD_ORD_CHANNEL_SUMS))
+            _lib.check(lib.dvd_bn_act_bwd_ordered(_ptr(g), _ptr(x), _ptr(y), _ptr(gamma), _ptr(mean), _ptr(var), ctx.eps, _ptr(gx),
+                                                  _ptr(gres), _ptr(gg), _ptr(gb), N * H * W, C, int(ctx.relu), *ws, _stream()),
+                       'dvd_bn_act_bwd_ordered')
+        else:
+            LAUNCHES['n'] += 1
+            _lib.check(lib.dvd_bn_act_bwd(_ptr(g), _ptr(x), _ptr(y), _ptr(gamma), _ptr(mean), _ptr(var), ctx.eps, _ptr(gx),
+                                          _ptr(gres), _ptr(gg), _ptr(gb), N * H * W, C, int(ctx.relu), _stream()), 'dvd_bn_act_bwd')
         if direct:
             return gx, gres, None, None, None, None, None, None
         return gx, gres, gg, gb, None, None, None, None

@@ -12,6 +12,8 @@ def add_general_arguments(parser):
     a = parser.add_argument
     a('--gpu', default='none', type=str, help="gpu to use ('-1' is rejected: dvd_b200 has no CPU path)")
     a('--manual_seed', type=int, default=None)
+    a('--deterministic', action='store_true',
+      help='bitwise reproducible training on one GPU: torch.use_deterministic_algorithms(True), ordered gradient reductions')
     a('--resume', type=int, default=0, help='0 scratch, -1 last checkpoint, -2 best, N epoch')
     a('--suffix', default='', type=str)
     a('--epoch', type=int, default=0, help='number of epochs to train')

@@ -67,6 +67,10 @@ def save_opt(opt):
 
 
 def main_worker(local_rank, ngpus, opt):
+    if opt.deterministic:
+        # before CUDA initialises: cuBLAS reads its workspace setting once, and torch raises on a cuBLAS call without it
+        os.environ.setdefault('CUBLAS_WORKSPACE_CONFIG', ':4096:8')
+        torch.use_deterministic_algorithms(True)
     env_world = int(os.environ.get('WORLD_SIZE', '1'))
     distributed = opt.multiprocess_distributed or env_world > 1
     if opt.gpu == '-1':

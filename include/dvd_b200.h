@@ -316,6 +316,55 @@ int dvd_head_fwd(const float* x, const float* w, const float* b, float* depth, l
 int dvd_head_bwd(const float* x, const float* w, const float* b, const float* g_depth, float* gx, float* gw, float* gb, long P,
                  int relu_mask, int round_out, void* stream);
 
+/* ---- ordered reductions: run-to-run reproducible backward kernels ---------------------------------------------------------
+ * Each *_ordered entry point takes the arguments of its namesake, then a workspace `ws` of `ws_bytes` bytes (16-byte aligned,
+ * any content), then the stream, and computes the same outputs without floating-point atomics: a CTA's partial sums go to a slab
+ * of the workspace and a second launch adds the slabs in a fixed order, so equal inputs give bitwise equal outputs on one GPU
+ * model. Launch geometry and split counts are those of the namesake. Launches that may run concurrently need workspaces of
+ * their own. dvd_ordered_workspace_bytes(site) is the size each site needs (0 for an unknown site); the re-projection
+ * backward's depends on the shape (dvd_reproject_ordered_bytes). See DESIGN.md 2.11.                                          */
+enum {
+  DVD_ORD_CONV_WGRAD = 0,    /* dvd_conv2d_wgrad_ordered */
+  DVD_ORD_MLP_WGRAD = 1,     /* dvd_mlp_wgrad_ordered */
+  DVD_ORD_MLP_DGRAD = 2,     /* dvd_mlp_dgrad_ordered */
+  DVD_ORD_CHANNEL_SUMS = 3,  /* dvd_relu_bwd_colsum_ordered, dvd_bn_act_bwd_ordered (C <= DVD_ORD_MAX_CHANNELS) */
+  DVD_ORD_STEM = 4,          /* dvd_stem_wgrad_ordered */
+  DVD_ORD_HEAD = 5           /* dvd_head_bwd_ordered */
+};
+#define DVD_ORD_CONV_MAX_CTAS 8192
+#define DVD_ORD_MAX_CHANNELS 8192
+size_t dvd_ordered_workspace_bytes(int site);
+size_t dvd_reproject_ordered_bytes(int B, int H, int W);
+int dvd_conv2d_wgrad_ordered(const dvd_conv_desc* desc, const float* x, const float* gy, float* dweight, const float* weight,
+                             long stride_co, long stride_ci, long stride_ky, long stride_kx, int ksize, int groups,
+                             const float* bn_gamma, const float* bn_var, float* dgamma, float* colsum, const float* bn_mean,
+                             void* ws, size_t ws_bytes, void* stream);
+int dvd_mlp_wgrad_ordered(const dvd_mlp_cfg* cfg, const void* save_e, const void* dy_scratch, float* const* g_w,
+                          float* const* g_b, long npx, void* ws, size_t ws_bytes, void* stream);
+int dvd_mlp_dgrad_ordered(const dvd_mlp_cfg* cfg, const void* packed_bwd, const float* p_e, const float* t0,
+                          float dt, int e, int use_g_acc, const float* g_acc, const float* g_step,
+                          const float* a_in, float* a_out, const void* save_e, void* dy_scratch,
+                          float* g_bias5, long npx, long hw, void* ws, size_t ws_bytes, void* stream);
+/* g_depth_2: each pixel's four bilinear taps are written as (target, contribution) pairs, sorted by target with a stable radix
+ * sort and summed run by run in pixel order.                                                                                   */
+int dvd_reproject_loss_bwd_ordered(const float* depth_1, const float* depth_2, const float* flow_1_2,
+                                   const float* mask_2, const float* sf, const float* poses,
+                                   const dvd_loss_cfg* cfg, const float* scalars, float gscale,
+                                   const float* gscale_dev, float* g_sf, float* g_depth_2,
+                                   int B, int H, int W, void* ws, size_t ws_bytes, void* stream);
+int dvd_relu_bwd_colsum_ordered(const float* g, const float* y, float* gm, float* colsum, const float* bn_mean,
+                                const float* bn_var, float bn_eps, float* dgamma, long P, int C, int round_out, void* ws,
+                                size_t ws_bytes, void* stream);
+int dvd_bn_act_bwd_ordered(const float* g, const float* x, const float* y, const float* gamma, const float* mean,
+                           const float* var, float eps, float* gx, float* gres, float* ggamma, float* gbeta,
+                           long P, int C, int relu, void* ws, size_t ws_bytes, void* stream);
+int dvd_stem_wgrad_ordered(const float* x_nchw, const float* g, const float* a0, const float* weight, float* dweight, long s_co,
+                           long s_ci, long s_ky, long s_kx, const float* bn_gamma, const float* bn_mean, const float* bn_var,
+                           float bn_eps, float* dgamma, float* dbeta, const float* norm_mean3, const float* norm_std3,
+                           float* scratch, int N, int H, int W, void* ws, size_t ws_bytes, void* stream);
+int dvd_head_bwd_ordered(const float* x, const float* w, const float* b, const float* g_depth, float* gx, float* gw, float* gb,
+                         long P, int relu_mask, int round_out, void* ws, size_t ws_bytes, void* stream);
+
 /* ---- flow-pair preprocessing (csrc/flow_pairs.cu): raw optical flows -> the training pair's flows and masks ------------------
  * scripts/preprocess/davis/generate_flows.py:44-82,139-148. Flows are NHWC fp32 [B,H,W,2] (the pair-file layout), 8-byte
  * aligned; every call checks its shapes, alignment and buffer byte sizes before it launches and returns -2 with a message.   */
