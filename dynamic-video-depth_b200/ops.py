@@ -1079,3 +1079,68 @@ def vis_tiles(maps, turbo, wheel):
     _lib.check(lib.dvd_vis_tiles(arr, len(maps), H, W, _ptr(ranges), _ptr(turbo), _ptr(wheel), _ptr(tiles), _stream()),
                'dvd_vis_tiles')
     return tiles
+
+
+# ---- novel views (csrc/render_views.cu) ---------------------------------------------------------------------------------------
+def view_keys(n, H, W, device):
+    """A key buffer for splat_views: [n,H,W] int64 (read as uint64 by the kernels), all ones, i.e. no point yet."""
+    return torch.full((n, H, W), -1, dtype=torch.int64, device=device)
+
+
+def splat_views(keys, xyz, cams, splat=1, index=None):
+    """dvd_splat_views: splats the points xyz [M,3] fp32 into the key buffer keys [F,H,W] int64 (view_keys) seen through cams
+    [F,21] fp32 (w2c 3x4 | K 3x3, row-major). With index [M] int64 (dvd_points_select's, chunk-relative: frame * H * W + pixel),
+    point p goes into view index[p] // (H W) only and carries its pixel index; without, every point goes into every view and
+    point r carries H W + r. Each pixel keeps the minimum key (bits(q2) << 32) | index, so repeated calls accumulate."""
+    _chk_dtype(keys, 'keys', torch.int64, 3)
+    F, H, W = keys.shape
+    _chk(cams, 'cams', (F, _lib.DVD_VIEW_CAM_FLOATS))
+    _chk(xyz, 'xyz')
+    if xyz.dim() != 2 or xyz.shape[1] != 3:
+        raise ValueError('xyz must be [M,3], got %s' % (tuple(xyz.shape),))
+    if not 1 <= int(splat) <= _lib.DVD_SPLAT_MAX:
+        raise ValueError('splat must be in [1, %d], got %r' % (_lib.DVD_SPLAT_MAX, splat))
+    if xyz.device != keys.device or cams.device != keys.device:
+        raise ValueError('keys, xyz and cams must be on one device')
+    M, HW = xyz.shape[0], H * W
+    if index is not None:
+        _chk_dtype(index, 'index', torch.int64, 1)
+        if index.shape[0] != M or index.device != keys.device:
+            raise ValueError('index must hold one entry per point (%d) on the points\' device' % M)
+        if M:
+            lo, hi = (int(v) for v in index.aminmax())
+            if lo < 0 or hi >= F * HW:
+                raise ValueError('index spans [%d, %d], outside the %d views of %dx%d pixels' % (lo, hi, F, H, W))
+    elif HW + M >= 2 ** 32:
+        raise ValueError('H W + %d static points = %d reach 2^32, beyond the 32-bit index of a key' % (M, HW + M))
+    LAUNCHES['n'] += 1
+    _lib.check(_lib.load().dvd_splat_views(_ptr(xyz), _ptr(index), M, _ptr(cams), F, H, W, int(splat), _ptr(keys), _stream()),
+               'dvd_splat_views')
+    return keys
+
+
+def resolve_views(keys, img, static_rgb=None, out=None, coverage=None):
+    """dvd_resolve_views: keys [F,H,W] of splat_views, img [F,3,H,W] fp32 of the views' own frames, static_rgb [R,3] uint8 RGB of
+    the static cloud splatted into them (None when there was none) -> (out [F,H,W,3] uint8 BGR, coverage [F] int32: the pixels
+    that received a point). Empty pixels are black. `out` and `coverage` may be given (e.g. views of one staging buffer)."""
+    _chk_dtype(keys, 'keys', torch.int64, 3)
+    F, H, W = keys.shape
+    _chk(img, 'img', (F, 3, H, W))
+    if static_rgb is not None:
+        _chk_dtype(static_rgb, 'static_rgb', torch.uint8, 2)
+        if static_rgb.shape[1] != 3 or static_rgb.device != keys.device:
+            raise ValueError('static_rgb must be [R,3] on the keys\' device, got %s' % (tuple(static_rgb.shape),))
+    if out is None:
+        out = torch.empty(F, H, W, 3, dtype=torch.uint8, device=keys.device)
+    _chk_dtype(out, 'out', torch.uint8, 4)
+    if tuple(out.shape) != (F, H, W, 3) or out.device != keys.device or img.device != keys.device:
+        raise ValueError('out must be [%d,%d,%d,3] and img on the keys\' device' % (F, H, W))
+    if coverage is None:
+        coverage = torch.empty(F, dtype=torch.int32, device=keys.device)
+    _chk_dtype(coverage, 'coverage', torch.int32, 1)
+    if coverage.shape[0] != F or coverage.device != keys.device:
+        raise ValueError('coverage must be [%d] on the keys\' device' % F)
+    LAUNCHES['n'] += 1
+    _lib.check(_lib.load().dvd_resolve_views(_ptr(keys), _ptr(img), _ptr(static_rgb), F, H, W, _ptr(out), _ptr(coverage), _stream()),
+               'dvd_resolve_views')
+    return out, coverage

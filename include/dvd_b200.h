@@ -454,6 +454,26 @@ int dvd_voxel_reduce(const long long* skey, const long long* order, const long l
                      long long M, long long hw, int min_views, double* mean_xyz, double* mean_rgb, int* count, int* views,
                      void* scratch, size_t scratch_bytes, long long* n_out, void* stream);
 
+/* ---- novel views of a test export (csrc/render_views.cu): point clouds splatted into virtual cameras. --------------------- */
+#define DVD_VIEW_CAM_FLOATS 21
+#define DVD_SPLAT_MAX 4
+/* cams [n_views, 21] fp32 per view: w2c (3 x 4 row-major: R^T | -R^T c) then K (3 x 3 row-major). keys [n_views, H, W] uint64,
+ * set to all ones by the caller before the first call of a chunk. Point p (xyz [n_points, 3] fp32) is projected with every
+ * operation rounded on its own, q_i = ((W_i0 P0 + W_i1 P1) + W_i2 P2) + t_i, h_i = (K_i0 q0 + K_i1 q1) + K_i2 q2, u = h0 / h2,
+ * v = h1 / h2, and dropped when q2 <= 1e-2f or a coordinate is not finite. It covers the splat x splat pixels from x0 = floor(u
+ * + 0.5f) - (splat - 1) / 2, y0 likewise, inside the image, and each covered pixel keeps min((bits(q2) << 32) | idx) (atomicMin).
+ * With index (int64 [n_points]): point p belongs to view index[p] / (H W) in [0, n_views) and idx = index[p] % (H W), its source
+ * pixel. With index NULL (a static cloud): every point is splatted into every view with idx = H W + p; H W + n_points must stay
+ * below 2^32 (-1 otherwise). 1 <= splat <= DVD_SPLAT_MAX. The keys are a pure function of the inputs, whatever the order.      */
+int dvd_splat_views(const float* xyz, const long long* index, long long n_points, const float* cams, int n_views, int H, int W,
+                    int splat, unsigned long long* keys, void* stream);
+/* keys [n_views, H, W] -> out [n_views, H, W, 3] uint8 BGR and coverage [n_views] int32 (pixels with a point). A pixel whose key
+ * is all ones is black; idx = the low 32 bits below H W takes the colour floor(255 clip(img[f, :, idx], 0, 1)) in fp32 (NaN -> 0;
+ * img [n_views, 3, H, W] fp32, dvd_points_select's colour rule), idx >= H W takes static_rgb[idx - H W] ([R, 3] uint8 RGB; may be
+ * NULL when no static point was splatted).                                                                                       */
+int dvd_resolve_views(const unsigned long long* keys, const float* img, const unsigned char* static_rgb, int n_views, int H, int W,
+                      unsigned char* out, int* coverage, void* stream);
+
 /* ---- test-end visualisation (csrc/test_videos.cu): models/video_base.py:157-272 (on_test_end) without matplotlib. ----------- */
 #define DVD_VIS_MAX_PANELS 4
 enum { DVD_VIS_DISP = 0, DVD_VIS_GT_DISP = 1, DVD_VIS_RGB = 2 };
