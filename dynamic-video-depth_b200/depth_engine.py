@@ -109,7 +109,16 @@ class MidasEngine:
 
     # ---------------------------------------------------------------------------------------------------
     def forward(self, x, train):
-        """x [N,3,H,W] raw image in [0,1] (contiguous fp32 CUDA) -> depth [N,1,H,W]. train=True keeps what backward needs."""
+        """x [N,3,H,W] raw image in [0,1] (contiguous fp32 CUDA) -> depth [N,1,H,W]. train=True keeps what backward needs.
+        H and W must be positive multiples of 32: layer4 runs at 1/32 of the image, and at any other size the x2 up-sampled
+        decoder path no longer matches the skip tensor it is added to (the convolution epilogue would read it with the wrong
+        strides). Checked before any launch."""
+        if x.dim() != 4 or x.shape[1] != 3:
+            raise ValueError('the MiDaS engine takes an image batch [N,3,H,W], got %s' % (tuple(x.shape),))
+        N, _, H, W = x.shape
+        if N < 1 or H < 32 or W < 32 or H % 32 or W % 32:
+            raise ValueError('the MiDaS engine runs at sizes whose height and width are positive multiples of 32, got %d x %d '
+                             '(batch %d)' % (H, W, N))
         self.pack(need_bwd=train)
         x = x.contiguous()
         nm, ns = (_NORM_MEAN, _NORM_STD) if self.normalize else (None, None)

@@ -42,8 +42,8 @@ of its id, and a missing key raises KeyError), so it is not built: a frame witho
 Deliberate deviations from the ShutterStock script, all ValueError:
   * a frame with no pixel where mvs > 1e-3 (the script gives s = NaN and NaN poses);
   * frames of one track with different stored sizes or MVS dtypes (the training data needs one working size);
-  * a stored size that is not a multiple of 32, which the MiDaS engine cannot run (the reference fails inside its decoder for
-    most such sizes and otherwise predicts depth at a larger size than the image);
+  * a stored size that is not a multiple of 32, which the MiDaS engine cannot run (MidasEngine.forward raises ValueError for
+    it; the reference fails inside its decoder for most such sizes and otherwise predicts depth at a larger size than the image);
   * a working size of 0 (a side under 32 where the script rounds down);
   * a prediction/img that is not fp32 [H,W,3].
 

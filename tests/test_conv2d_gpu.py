@@ -81,6 +81,24 @@ FWD_CASES = [
     (2, 14, 24, 256, 256, 3, 1, 1, False, True, True, True, True, False),      # few tiles, 72 K-steps: tiles split four ways
     (1, 20, 36, 64, 64, 5, 1, 1, False, True, False, False, True, False),      # 5x5 (hourglass class): 25 taps
     (1, 24, 40, 32, 32, 11, 1, 1, False, True, False, False, True, False),     # 11x11: 121 taps
+    # layer4 of the working sizes with a one-row, one-column or single-pixel layer4 grid (32 x 384, 384 x 32, 32 x 32 images):
+    # a 128 x 1 or 8 x 16 pixel tile (TMA box wider or taller than the tensor) of which the epilogue keeps 12 pixels, or 1
+    (2, 1, 12, 2048, 256, 3, 1, 1, False, True, False, False, True, False),    # layer4_rn, 1 x 12
+    (2, 12, 1, 2048, 256, 3, 1, 1, False, True, False, False, True, False),    # layer4_rn, 12 x 1
+    (4, 1, 1, 2048, 256, 3, 1, 1, False, True, False, False, True, False),     # layer4_rn, 1 x 1
+    (2, 1, 12, 1024, 2048, 1, 1, 1, True, False, True, False, True, False),    # 1x1 1024 -> 2048 (one GEMM over 24 pixels)
+    (2, 12, 1, 1024, 2048, 1, 1, 1, True, False, True, False, True, False),
+    (4, 1, 1, 1024, 2048, 1, 1, 1, True, False, True, False, True, False),     # 4 pixels
+    (2, 2, 24, 1024, 1024, 3, 2, 32, True, False, False, False, True, False),  # grouped stride 2, 32 ch / group -> 1 x 12
+    (2, 24, 2, 1024, 1024, 3, 2, 32, True, False, False, False, True, False),  # -> 12 x 1
+    (4, 2, 2, 1024, 1024, 3, 2, 32, True, False, False, False, True, False),   # -> 1 x 1
+    (2, 2, 24, 2048, 2048, 3, 2, 32, True, False, False, False, True, False),  # layer4.0.conv2 (64 ch / group) -> 1 x 12
+    (2, 24, 2, 2048, 2048, 3, 2, 32, True, False, False, False, True, False),  # -> 12 x 1
+    (4, 2, 2, 2048, 2048, 3, 2, 32, True, False, False, False, True, False),   # -> 1 x 1
+    (2, 2, 24, 1024, 2048, 1, 2, 1, True, False, False, False, False, False),  # layer4.0.downsample, 1x1 stride 2 -> 1 x 12
+    (2, 24, 2, 1024, 2048, 1, 2, 1, True, False, False, False, False, False),  # -> 12 x 1
+    (4, 2, 2, 1024, 2048, 1, 2, 1, True, False, False, False, False, False),   # -> 1 x 1
+    (1, 1, 1, 2048, 256, 3, 1, 1, False, True, True, True, True, False),       # one tile of one pixel, 576 K-steps: stream-K over 4 CTAs
 ]
 
 
@@ -261,6 +279,22 @@ DGRAD_CASES = [
     (2, 56, 96, 512, 512, 3, 2, 32, True, False, True),      # grouped stride 2: four sub-pixel phases + mask
     (1, 27, 45, 256, 256, 3, 2, 32, True, True, False),      # odd sizes + residual
     (1, 20, 36, 64, 64, 7, 1, 1, False, False, False),       # 7x7
+    # layer4 classes at the one-row, one-column and single-pixel grids (see FWD_CASES)
+    (2, 1, 12, 2048, 256, 3, 1, 1, False, True, True),       # layer4_rn
+    (2, 12, 1, 2048, 256, 3, 1, 1, False, True, True),
+    (4, 1, 1, 2048, 256, 3, 1, 1, False, True, True),
+    (2, 1, 12, 1024, 2048, 1, 1, 1, True, True, True),       # 1x1 1024 -> 2048
+    (4, 1, 1, 1024, 2048, 1, 1, 1, True, True, True),
+    (2, 2, 24, 1024, 1024, 3, 2, 32, True, False, True),     # grouped stride 2, 32 ch / group: 1 x 12 -> 2 x 24
+    (2, 24, 2, 1024, 1024, 3, 2, 32, True, True, False),     # 12 x 1 -> 24 x 2
+    (4, 2, 2, 1024, 1024, 3, 2, 32, True, False, True),      # 1 x 1 -> 2 x 2
+    (2, 2, 24, 2048, 2048, 3, 2, 32, True, False, True),     # 64 ch / group
+    (4, 2, 2, 2048, 2048, 3, 2, 32, True, True, False),
+    (2, 2, 24, 1024, 2048, 1, 2, 1, True, False, False),     # 1x1 stride-2 downsample: zero fill + one phase
+    (2, 24, 2, 1024, 2048, 1, 2, 1, True, False, False),
+    (4, 2, 2, 1024, 2048, 1, 2, 1, True, False, False),
+    (1, 1, 1, 2048, 256, 3, 1, 1, False, True, True),        # layer4_rn's data gradient at one pixel: 8 tiles of 72 K-steps
+    (1, 1, 1, 256, 2048, 3, 1, 1, False, True, True),        # launch Cin 2048: one tile, 576 K-steps, stream-K over 4 CTAs
 ]
 
 
@@ -307,6 +341,20 @@ WGRAD_CASES = [
     (1, 14, 24, 512, 512, 3, 1, 32, True),       # 16
     (1, 14, 24, 1024, 1024, 3, 1, 32, False),    # 32
     (1, 7, 12, 2048, 2048, 3, 1, 32, True),      # 64
+    # layer4 classes at the one-row, one-column and single-pixel grids (see FWD_CASES)
+    (2, 1, 12, 2048, 256, 3, 1, 1, False),       # layer4_rn
+    (2, 12, 1, 2048, 256, 3, 1, 1, False),
+    (4, 1, 1, 2048, 256, 3, 1, 1, False),
+    (2, 1, 12, 1024, 2048, 1, 1, 1, True),       # 1x1 1024 -> 2048
+    (4, 1, 1, 1024, 2048, 1, 1, 1, True),
+    (2, 2, 24, 1024, 1024, 3, 2, 32, True),      # grouped stride 2, 32 ch / group
+    (2, 24, 2, 1024, 1024, 3, 2, 32, True),
+    (4, 2, 2, 1024, 1024, 3, 2, 32, True),
+    (2, 2, 24, 2048, 2048, 3, 2, 32, True),      # 64 ch / group
+    (4, 2, 2, 2048, 2048, 3, 2, 32, True),
+    (2, 2, 24, 1024, 2048, 1, 2, 1, True),       # 1x1 stride-2 downsample
+    (2, 24, 2, 1024, 2048, 1, 2, 1, True),
+    (4, 2, 2, 1024, 2048, 1, 2, 1, True),
 ]
 
 

@@ -27,7 +27,8 @@ POOL_FLIPS = 1e-4       # max-pool argmax of the emulated window (first maximum)
 # forward, unrounded tensors (down-sample branch outputs, h2, depth): max-norm relative to the tensor's maximum; observed 3.1e-6
 UNROUNDED_REL = 1e-5
 # backward, every parameter tensor: |slope - 1|, relative L2, max-norm relative to the tensor's maximum;
-#   observed maxima 3.3e-4 (layer2.0.bn2.weight), 1.07e-3 (layer3.3.bn2.weight), 1.8e-3 (layer3.4.bn1.weight)
+#   observed maxima 3.3e-4 (layer2.0.bn2.weight), 1.07e-3 (layer3.3.bn2.weight), 1.8e-3 (layer3.4.bn1.weight); at the working
+#   sizes 3.2e-4 (1x384x224), 1.41e-3 (2x64x384), 2.3e-3 (2x32x384, layer3.0.bn1.weight)
 GRAD_SLOPE, GRAD_L2, GRAD_MAX = 1e-3, 3e-3, 5e-3
 # data-gradient images: share of elements one TF32 step away from tf32(W * gamma * rsqrt(var + eps)) where rsqrtf and
 # torch.rsqrt differ; observed 0 of 8.7e7
@@ -189,8 +190,31 @@ def _check_engine_against_emulation(N, H, W, kind):
                                    {k: p.grad for k, p in net.named_parameters()}, '%dx%dx%d %s' % (N, H, W, kind))
 
 
-@pytest.mark.parametrize('kind', ['smooth', 'white'])
-@pytest.mark.parametrize('shape', [(2, 64, 96), (1, 224, 384)])
+# The working sizes the frame builders produce (frames.working_size, frames.get_im_size), with their layer4 grids: 16:9 and 4:3
+# videos (6 x 12, 8 x 12), a portrait phone video (22 x 12: the tallest activations the engine runs, 3.1x the pixels of
+# 224 x 384 per image), a square one (12 x 12), a very wide COLMAP video (2 x 12), a ShutterStock portrait (12 x 7), very wide /
+# very tall ShutterStock frames (1 x 12 / 12 x 1: one-row and one-column grids) and small ones (1 x 1). The emulation needs about
+# 2.2 GB per 224 x 384 image, in proportion to the pixels: the large sizes carry a timeout like the bench-resolution test.
+_LARGE = pytest.mark.timeout(1200)
+ENGINE_CASES = [
+    pytest.param((2, 64, 96), 'smooth', id='shape0-smooth'),
+    pytest.param((2, 64, 96), 'white', id='shape0-white'),
+    pytest.param((1, 224, 384), 'smooth', id='shape1-smooth'),
+    pytest.param((1, 224, 384), 'white', id='shape1-white'),
+    pytest.param((2, 192, 384), 'white', id='2x192x384-white', marks=_LARGE),
+    pytest.param((2, 256, 384), 'white', id='2x256x384-white', marks=_LARGE),
+    pytest.param((1, 704, 384), 'white', id='1x704x384-white', marks=_LARGE),
+    pytest.param((1, 384, 384), 'white', id='1x384x384-white', marks=_LARGE),
+    pytest.param((2, 64, 384), 'white', id='2x64x384-white'),
+    pytest.param((1, 384, 224), 'white', id='1x384x224-white', marks=_LARGE),
+    pytest.param((1, 384, 224), 'smooth', id='1x384x224-smooth', marks=_LARGE),
+    pytest.param((2, 32, 384), 'white', id='2x32x384-white'),
+    pytest.param((2, 384, 32), 'white', id='2x384x32-white'),
+    pytest.param((4, 32, 32), 'white', id='4x32x32-white'),
+]
+
+
+@pytest.mark.parametrize('shape, kind', ENGINE_CASES)
 def test_saved_tensors_match_tf32_emulation(shape, kind, monkeypatch):
     monkeypatch.delenv('DVD_BWD_OVERLAP', raising=False)
     _check_engine_against_emulation(*shape, kind)

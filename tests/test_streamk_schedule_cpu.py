@@ -57,7 +57,17 @@ def _check(ntiles, ksteps, n):
         assert pos == ksteps
 
 
-@pytest.mark.parametrize('shape', [(84, 32, 74), (6, 576, 74), (24, 288, 74), (1, 64, 4), (48, 64, 74), (168, 16, 74), (11, 8, 11), (3, 9, 2)])
+# (tiles, K-steps, CTAs). The H100 launch runs one CTA per SM (up to 132) and at most max(8, K-steps / 4) K-steps per range:
+#   layer4_rn (3x3, 2048 -> 256, one 256-channel tile per image) at the bench batch 16 x 7 x 12: 16 tiles over 64 CTAs;
+#   at the 1 x 12 / 12 x 1 layer4 grids of 32 x 384 / 384 x 32 images (one tile per image): 2 tiles over 8 CTAs;
+#   at the 1 x 1 grid of a 32 x 32 image: 1 tile over 4 CTAs (4 images: 4 tiles over 16);
+#   layer3_rn (3x3, 1024 -> 256) at the bench batch 16 x 14 x 24: 48 tiles, 288 K-steps over 132 CTAs;
+#   the data gradient of a 3x3 256 -> 2048 convolution at a 1 x 1 grid (2048 input channels): 1 tile over 4 CTAs.
+H100_LAYERS = [(16, 576, 64), (2, 576, 8), (1, 576, 4), (4, 576, 16), (48, 288, 132), (132, 576, 132), (133, 1152, 132)]
+
+
+@pytest.mark.parametrize('shape', [(84, 32, 74), (6, 576, 74), (24, 288, 74), (1, 64, 4), (48, 64, 74), (168, 16, 74), (11, 8, 11),
+                                   (3, 9, 2)] + H100_LAYERS)
 def test_partition_of_the_layers_of_the_depth_net(shape):
     _check(*shape)
 
@@ -66,7 +76,7 @@ def test_partition_invariants_on_random_shapes():
     rnd = random.Random(0)
     done = 0
     while done < 3000:
-        ks, n, nt = rnd.randint(1, 130), rnd.randint(1, 74), rnd.randint(1, 400)
+        ks, n, nt = rnd.randint(1, 1152), rnd.randint(1, 132), rnd.randint(1, 400)
         if nt * ks < n:
             continue
         _check(nt, ks, n)
