@@ -64,6 +64,7 @@ DVD_VIS_DISP, DVD_VIS_GT_DISP, DVD_VIS_RGB = 0, 1, 2
 DVD_VIS_MAX_PANELS = 4
 DVD_VIEW_CAM_FLOATS = 21
 DVD_SPLAT_MAX = 4
+DVD_REFOCUS_MAX_RADIUS = 32
 
 
 class VisMap(ctypes.Structure):
@@ -179,6 +180,7 @@ SIGNATURES = {
     'dvd_vis_panels': [_P, _L, _I, _I, _I, ctypes.POINTER(VisPanel), _I, _P, _P, _P],
     'dvd_splat_views': [_P, _P, _L, _P, _I, _I, _I, _I, _P, _P],
     'dvd_resolve_views': [_P, _P, _P, _I, _I, _I, _P, _P, _P],
+    'dvd_refocus': [_P, _P, _P, _F, _I, _P, _I, _I, _I, _P],
     'dvd_vis_ranges': [ctypes.POINTER(VisMap), _I, _I, _I, _P, _P],
     'dvd_vis_tiles': [ctypes.POINTER(VisMap), _I, _I, _I, _P, _P, _P, _P, _P],
 }

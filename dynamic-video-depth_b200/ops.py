@@ -1144,3 +1144,33 @@ def resolve_views(keys, img, static_rgb=None, out=None, coverage=None):
     _lib.check(_lib.load().dvd_resolve_views(_ptr(keys), _ptr(img), _ptr(static_rgb), F, H, W, _ptr(out), _ptr(coverage), _stream()),
                'dvd_resolve_views')
     return out, coverage
+
+
+# ---- synthetic depth of field (csrc/refocus.cu) -------------------------------------------------------------------------------
+def refocus(depth, img, focus_disp, scale, max_radius, out=None):
+    """dvd_refocus: frames depth [N,H,W] fp32 and img [N,3,H,W] fp32 RGB, blurred by each pixel's blur radius
+    c = min(max_radius, scale |disp - focus_disp[n]|) with the exact gather rule of include/dvd_b200.h -> out [N,H,W,3] uint8
+    BGR (which may be given, e.g. a view of a staging buffer). focus_disp [N] fp32 is the frames' focal disparities; scale is
+    a finite fp32 >= 0 and 0 <= max_radius <= 32. With scale 0 or max_radius 0 the frames come out as floor(255 clip(img))."""
+    _chk(depth, 'depth')
+    if depth.dim() != 3:
+        raise ValueError('depth must be [N,H,W], got %s' % (tuple(depth.shape),))
+    N, H, W = depth.shape
+    _chk(img, 'img', (N, 3, H, W))
+    _chk(focus_disp, 'focus_disp', (N,))
+    if not 0 <= int(max_radius) <= _lib.DVD_REFOCUS_MAX_RADIUS or int(max_radius) != max_radius:
+        raise ValueError('max_radius must be an integer in [0, %d], got %r' % (_lib.DVD_REFOCUS_MAX_RADIUS, max_radius))
+    scale = float(scale)
+    if not (scale >= 0 and scale < float('inf')):
+        raise ValueError('scale must be finite and >= 0, got %r' % scale)
+    if not 1 <= N <= 65535:
+        raise ValueError('refocus takes 1 to 65535 frames per call, got %d' % N)
+    if out is None:
+        out = torch.empty(N, H, W, 3, dtype=torch.uint8, device=depth.device)
+    _chk_dtype(out, 'out', torch.uint8, 4)
+    if tuple(out.shape) != (N, H, W, 3) or not (out.device == img.device == focus_disp.device == depth.device):
+        raise ValueError('out must be [%d,%d,%d,3], and every tensor on one device' % (N, H, W))
+    LAUNCHES['n'] += 1
+    _lib.check(_lib.load().dvd_refocus(_ptr(depth), _ptr(img), _ptr(focus_disp), scale, int(max_radius), _ptr(out), N, H, W,
+                                       _stream()), 'dvd_refocus')
+    return out

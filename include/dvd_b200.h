@@ -474,6 +474,18 @@ int dvd_splat_views(const float* xyz, const long long* index, long long n_points
 int dvd_resolve_views(const unsigned long long* keys, const float* img, const unsigned char* static_rgb, int n_views, int H, int W,
                       unsigned char* out, int* coverage, void* stream);
 
+/* ---- synthetic depth of field (csrc/refocus.cu): a test export's frames blurred by their distance from a focal plane. --- */
+#define DVD_REFOCUS_MAX_RADIUS 32
+/* depth [N, H, W] fp32, img [N, 3, H, W] fp32 RGB, focus_disp [N] fp32 (device) -> out [N, H, W, 3] uint8 BGR. Every operation
+ * is fp32 and rounded on its own. Per pixel: disp = 1 / d when d is finite and > 1e-2f, else 0; c = min(max_radius, scale
+ * |disp - focus_disp[n]|); col = clip(img, 0, 1) per channel with NaN -> 0. For every tap (dx, dy) with dx^2 + dy^2 <=
+ * max_radius^2, dy ascending then dx, whose q = p + (dx, dy) lies in the image: r = sqrt(dx^2 + dy^2), ce = disp(q) < disp(p) ?
+ * min(c(q), c(p)) : c(q), w = clamp(ce - r + 0.5, 0, 1) / max(ce^2, 0.25); S_k += w col_k(q), W += w in tap order. out =
+ * min(255, floor(255 (S_k / W))). 0 <= max_radius <= DVD_REFOCUS_MAX_RADIUS and a finite scale >= 0, else -2. The output is a
+ * pure function of the inputs; with c = 0 everywhere it is floor(255 col).                                                     */
+int dvd_refocus(const float* depth, const float* img, const float* focus_disp, float scale, int max_radius, unsigned char* out,
+                int N, int H, int W, void* stream);
+
 /* ---- test-end visualisation (csrc/test_videos.cu): models/video_base.py:157-272 (on_test_end) without matplotlib. ----------- */
 #define DVD_VIS_MAX_PANELS 4
 enum { DVD_VIS_DISP = 0, DVD_VIS_GT_DISP = 1, DVD_VIS_RGB = 2 };
