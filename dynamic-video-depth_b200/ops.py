@@ -1174,3 +1174,97 @@ def refocus(depth, img, focus_disp, scale, max_radius, out=None):
     _lib.check(_lib.load().dvd_refocus(_ptr(depth), _ptr(img), _ptr(focus_disp), scale, int(max_radius), _ptr(out), N, H, W,
                                        _stream()), 'dvd_refocus')
     return out
+
+
+# ---- evaluation of a test export (csrc/depth_metrics.cu) ----------------------------------------------------------------------
+def _same_device(name, *ts):
+    if len({t.device for t in ts if t is not None}) != 1:
+        raise ValueError('%s: every tensor must be on one device' % name)
+
+
+def masked_select_median(values, other=None):
+    """dvd_masked_select: values [N,H,W] fp32 (and other of the same shape, or None) -> (median [N+1] fp32, count [N+1] int64):
+    per frame and then over all frames pooled, the lower median (0-based rank (n - 1) // 2, exact) of the elements where values
+    (and other) are finite and > 1e-2; NaN with count 0 for an empty set."""
+    _chk(values, 'values')
+    if values.dim() != 3:
+        raise ValueError('values must be [N,H,W], got %s' % (tuple(values.shape),))
+    N, H, W = values.shape
+    if other is not None:
+        _chk(other, 'other', (N, H, W))
+    _same_device('masked_select_median', values, other)
+    if not 1 <= N <= 65535:
+        raise ValueError('masked_select_median takes 1 to 65535 frames per call, got %d' % N)
+    lib = _lib.load()
+    work = torch.empty(lib.dvd_masked_select_partials_size(N, H, W), dtype=torch.int64, device=values.device)
+    med = torch.empty(N + 1, dtype=torch.float32, device=values.device)
+    cnt = torch.empty(N + 1, dtype=torch.int64, device=values.device)
+    LAUNCHES['n'] += 9
+    _lib.check(lib.dvd_masked_select(_ptr(values), _ptr(other), _ptr(med), _ptr(cnt), _ptr(work), N, H, W, _stream()),
+               'dvd_masked_select')
+    return med, cnt
+
+
+DEPTH_METRIC_SLOTS = 22      # per source: count, then per scale |d'-g|/g, (d'-g)^2/g, (d'-g)^2, (ln d'-ln g)^2, three delta counts
+
+
+def depth_metrics(depth, depth_nn, depth_gt, scales):
+    """dvd_depth_metrics: depth, depth_nn, depth_gt [N,H,W] fp32 and scales [N,2,3] fp64 -> sums [N,2,22] fp64 (the layout of
+    include/dvd_b200.h): every frame's accuracy sums for both depth sources under the three scales."""
+    _chk(depth, 'depth')
+    if depth.dim() != 3:
+        raise ValueError('depth must be [N,H,W], got %s' % (tuple(depth.shape),))
+    N, H, W = depth.shape
+    _chk(depth_nn, 'depth_nn', (N, H, W))
+    _chk(depth_gt, 'depth_gt', (N, H, W))
+    _chk_dtype(scales, 'scales', torch.float64, 3)
+    if tuple(scales.shape) != (N, 2, 3):
+        raise ValueError('scales must be [%d,2,3], got %s' % (N, tuple(scales.shape)))
+    _same_device('depth_metrics', depth, depth_nn, depth_gt, scales)
+    if not 1 <= N <= 65535:
+        raise ValueError('depth_metrics takes 1 to 65535 frames per call, got %d' % N)
+    lib = _lib.load()
+    partials = torch.empty(lib.dvd_depth_metrics_partials_size(N, H, W), dtype=torch.float64, device=depth.device)
+    sums = torch.empty(N, 2, DEPTH_METRIC_SLOTS, dtype=torch.float64, device=depth.device)
+    LAUNCHES['n'] += 2
+    _lib.check(lib.dvd_depth_metrics(_ptr(depth), _ptr(depth_nn), _ptr(depth_gt), _ptr(scales), _ptr(sums), _ptr(partials), N, H,
+                                     W, _stream()), 'dvd_depth_metrics')
+    return sums
+
+
+PAIR_SLOTS = 6               # per source and region: count, behind, sum e_r, sum e_d, #e_r < 1, #e_r < 3
+
+
+def pair_consistency(depth, depth_nn, cam, ia, ib, flow, mask, motion_seg=None):
+    """dvd_pair_consistency: resident frames depth, depth_nn [F,H,W] fp32 and cam [F,30] fp32 (points.camera_block), pairs
+    ia, ib [P] int32 frame indices, flow [P,H,W,2] fp32 (flow_1_2), mask [P,H,W] uint8 (flowpair mask_2, 0 = good), motion_seg
+    [F,H,W] uint8 or None -> sums [P,2,2,6] fp64 per source (depth, depth_nn) and region (all, static)."""
+    _chk(depth, 'depth')
+    if depth.dim() != 3:
+        raise ValueError('depth must be [F,H,W], got %s' % (tuple(depth.shape),))
+    F, H, W = depth.shape
+    _chk(depth_nn, 'depth_nn', (F, H, W))
+    _chk(cam, 'cam', (F, 30))
+    _chk_dtype(ia, 'ia', torch.int32, 1)
+    P = ia.shape[0]
+    _chk_dtype(ib, 'ib', torch.int32, 1)
+    _chk(flow, 'flow', (P, H, W, 2))
+    _chk_dtype(mask, 'mask', torch.uint8, 3)
+    if tuple(ib.shape) != (P,) or tuple(mask.shape) != (P, H, W):
+        raise ValueError('ib must be [%d] and mask [%d,%d,%d], got %s and %s' % (P, P, H, W, tuple(ib.shape), tuple(mask.shape)))
+    if motion_seg is not None:
+        _chk_dtype(motion_seg, 'motion_seg', torch.uint8, 3)
+        if tuple(motion_seg.shape) != (F, H, W):
+            raise ValueError('motion_seg must be [%d,%d,%d], got %s' % (F, H, W, tuple(motion_seg.shape)))
+    _same_device('pair_consistency', depth, depth_nn, cam, ia, ib, flow, mask, motion_seg)
+    if not 1 <= P <= 65535:
+        raise ValueError('pair_consistency takes 1 to 65535 pairs per call, got %d' % P)
+    if int(ia.min()) < 0 or int(ib.min()) < 0 or int(ia.max()) >= F or int(ib.max()) >= F:
+        raise ValueError('pair frame indices must lie in [0, %d)' % F)
+    lib = _lib.load()
+    partials = torch.empty(lib.dvd_pair_consistency_partials_size(P, H, W), dtype=torch.float64, device=depth.device)
+    sums = torch.empty(P, 2, 2, PAIR_SLOTS, dtype=torch.float64, device=depth.device)
+    LAUNCHES['n'] += 2
+    _lib.check(lib.dvd_pair_consistency(_ptr(depth), _ptr(depth_nn), _ptr(cam), F, _ptr(ia), _ptr(ib), _ptr(flow), _ptr(mask),
+                                        _ptr(motion_seg), _ptr(sums), _ptr(partials), P, H, W, _stream()), 'dvd_pair_consistency')
+    return sums

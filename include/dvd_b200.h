@@ -486,6 +486,42 @@ int dvd_resolve_views(const unsigned long long* keys, const float* img, const un
 int dvd_refocus(const float* depth, const float* img, const float* focus_disp, float scale, int max_radius, unsigned char* out,
                 int N, int H, int W, void* stream);
 
+/* ---- evaluation of a test export (csrc/depth_metrics.cu): depth accuracy against depth_gt and consistency along the flow. ----
+ * A depth is valid when it is finite and > 1e-2f. Per-pixel arithmetic is fp64 after the fp32 load, every operation rounded on
+ * its own in the order written here; sums are fp64 in a fixed order (block partials in `partials`, then added in block order)
+ * and a frame's (pair's) sums do not depend on the other frames (pairs) of the launch: bitwise reproducible. The *_size queries
+ * return the number of 8-byte words of the workspace (-1 for a bad shape). Argument errors return -2 with a message.
+ *
+ * dvd_masked_select: values [N,H,W] fp32; element i of frame n is selected when values[n,i] is valid and, unless other is NULL,
+ * other[n,i] (same shape) is valid too. median [N+1] fp32 receives, per frame and then for all frames pooled, the lower median:
+ * the selected element of 0-based rank (n - 1) / 2, exact (radix select on order-preserving keys), NaN when n = 0; count [N+1]
+ * int64 receives n. work: int64 words.                                                                                     */
+long long dvd_masked_select_partials_size(int N, int H, int W);
+int dvd_masked_select(const float* values, const float* other, float* median, long long* count, long long* work, int N, int H,
+                      int W, void* stream);
+/* dvd_depth_metrics: depth, depth_nn, depth_gt [N,H,W] fp32, scales [N,2,3] fp64 (per frame, per source s = 0 depth, 1
+ * depth_nn, three depth scales a) -> sums [N,2,22] fp64. A pixel counts for source s when depth_gt g and the source's depth d are
+ * valid; with d' = scales[n,s,a]·d: sums[n,s,0] = count, and sums[n,s,1 + 7a + k] for k = 0..6: Σ |d' - g| / g, Σ (d' - g)² / g,
+ * Σ (d' - g)², Σ (ln d' - ln g)², and the counts of max(d' / g, g / d') < 1.25, 1.25², 1.25³. partials: fp64 words.          */
+long long dvd_depth_metrics_partials_size(int N, int H, int W);
+int dvd_depth_metrics(const float* depth, const float* depth_nn, const float* depth_gt, const double* scales, double* sums,
+                      double* partials, int N, int H, int W, void* stream);
+/* dvd_pair_consistency: depth, depth_nn [n_frames,H,W] fp32 and cam [n_frames,30] fp32 (K^T | (K^-1)^T | R | t, R t the
+ * camera-to-world pose: dvd_b200.points.camera_block) of resident frames; pair p runs from frame a = ia[p] to b = ib[p] (int32
+ * indices) with flow [n_pairs,H,W,2] fp32 (8-byte aligned) = flow_1_2 and mask [n_pairs,H,W] uint8 = the flowpair mask_2 (0 =
+ * good); motion_seg [n_frames,H,W] uint8 or NULL. A pixel x = (i, j) of a (column, row) is evaluated for a source D when mask is
+ * 0, q = x + flow is finite, D_a(x) is valid and so are the four bilinear taps of D_b at q: q clamped to [0, W-1] x [0, H-1],
+ * taps at (x0, y0) = floor, x1 = min(x0 + 1, W - 1), y1 = min(y0 + 1, H - 1), weights wx1 = qx - x0, wx0 = 1 - wx1 (y alike),
+ * D~ = ((wy0 wx0 D00 + wy0 wx1 D01) + wy1 wx0 D10) + wy1 wx1 D11. P = R_a (D_a(x) Kinv_a (i, j, 1)) + t_a, c = R_b^T (P - t_b)
+ * (each matrix row a left-to-right dot product; P - t_b formed after P); z = c.z. z <= 1e-3 counts as behind; otherwise
+ * p = (K_b c).xy / z, e_r = |p - q|, e_d = |z - D~| / D~. sums [n_pairs,2,2,6] fp64 per source (0 depth, 1 depth_nn) and
+ * region (0 all, 1 static: motion_seg of frame a is 0; zero without motion_seg): evaluated pixels not behind, behind, Σ e_r,
+ * Σ e_d, #e_r < 1, #e_r < 3. partials: fp64 words.                                                                          */
+long long dvd_pair_consistency_partials_size(int n_pairs, int H, int W);
+int dvd_pair_consistency(const float* depth, const float* depth_nn, const float* cam, int n_frames, const int* ia, const int* ib,
+                         const float* flow, const unsigned char* mask, const unsigned char* motion_seg, double* sums,
+                         double* partials, int n_pairs, int H, int W, void* stream);
+
 /* ---- test-end visualisation (csrc/test_videos.cu): models/video_base.py:157-272 (on_test_end) without matplotlib. ----------- */
 #define DVD_VIS_MAX_PANELS 4
 enum { DVD_VIS_DISP = 0, DVD_VIS_GT_DISP = 1, DVD_VIS_RGB = 2 };
