@@ -6,8 +6,8 @@ accurate. This measures both, for the refined `depth` and for the initial `depth
 and writes OUT/metrics.json, OUT/frames.csv (one row per frame) and OUT/pairs.csv (one row per pair); OUT defaults to
 --test_dir. It prints a refined-versus-initial table.
 
-Frames. The export's frames are read in file order (export_points.Frames: depth, K, cam_c2w, with points.camera_block's
-conventions) with their `depth_nn`, `depth_gt` and `pair_path`. A frame's number is the N of its pair_path basename
+Frames. The export's frames are read in file order (export_io.Frames: depth, depth_nn, depth_gt, K and cam_c2w, the
+poses with points.camera_block's conventions, and pair_path). A frame's number is the N of its pair_path basename
 `frame_N.npz`, else its position in the export.
 
 Accuracy against depth_gt, per frame and over the sequence. A pixel counts when depth_gt g and the evaluated depth d are valid
@@ -44,11 +44,12 @@ import numpy as np
 import torch
 
 from . import ops
-from .export_points import Frames, list_files
+from .export_io import Frames, chunk_size, cuda_device, list_files
 from .flow_pairs import PairBuilder, pair_list, read_npz
 from .points import camera_block
 
 F32 = np.float32
+KEYS = ('depth', 'depth_nn', 'depth_gt', 'img_1', 'K', 'cam_c2w')
 SOURCES = ('refined', 'initial')                 # depth, depth_nn
 ALIGNMENTS = ('none', 'frame', 'sequence')
 ACC_METRICS = ('abs_rel', 'sq_rel', 'rmse', 'rmse_log', 'd1', 'd2', 'd3')
@@ -65,34 +66,16 @@ def frame_number(pair_path, position):
 
 
 class Export:
-    """The frames of a test export in file order: depth, depth_nn, depth_gt [N,H,W] fp32, cam [N,30] fp32 (camera_block) and
-    the frame numbers."""
+    """The frames of a test export in file order (export_io.Frames, each file opened once): depth, depth_nn, depth_gt
+    [N,H,W] fp32, cam [N,30] fp32 (camera_block) and the frame numbers."""
 
     def __init__(self, test_dir):
-        fr = Frames(list_files(test_dir))
-        self.files, self.N, self.H, self.W = fr.files, fr.N, fr.H, fr.W
-        self.depth = fr.depth
-        self.cam = camera_block(fr.K, fr.c2w)
-        extra = {'depth_nn': [], 'depth_gt': []}
-        paths = []
-        for f in fr.files:
-            z = np.load(f)
-            B = None
-            for k in extra:
-                if k not in z.files:
-                    raise ValueError('%s lacks %s' % (f, k))
-                a = np.asarray(z[k], dtype=F32)
-                if a.ndim != 4 or a.shape[1] != 1 or a.shape[2:] != (self.H, self.W):
-                    raise ValueError('%s: %s must be [B,1,%d,%d], got %s' % (f, k, self.H, self.W, a.shape))
-                extra[k].append(a[:, 0])
-                B = a.shape[0]
-            pp = [str(p) for p in np.asarray(z['pair_path']).reshape(-1)] if 'pair_path' in z.files else []
-            paths += pp if len(pp) == B else [None] * B
-        self.depth_nn, self.depth_gt = (np.concatenate(extra[k]) for k in ('depth_nn', 'depth_gt'))
-        if self.depth_nn.shape != self.depth.shape or self.depth_gt.shape != self.depth.shape:
-            raise ValueError('depth_nn %s / depth_gt %s do not match depth %s' % (self.depth_nn.shape, self.depth_gt.shape,
-                                                                                 self.depth.shape))
-        self.numbers = np.asarray([frame_number(p, i) if p is not None else i for i, p in enumerate(paths)], dtype=np.int64)
+        ex = Frames(list_files(test_dir), keys=KEYS, optional=('pair_path',))
+        self.N, self.H, self.W = ex.N, ex.H, ex.W
+        self.depth, self.depth_nn, self.depth_gt = ex.depth, ex.depth_nn, ex.depth_gt
+        self.cam = camera_block(ex.K, ex.c2w)
+        self.numbers = np.asarray([frame_number(p, i) if p is not None else i for i, p in enumerate(ex.pair_path)],
+                                  dtype=np.int64)
         if len(set(self.numbers.tolist())) != self.N:
             raise ValueError('the frames of %s do not have distinct numbers' % test_dir)
 
@@ -223,11 +206,9 @@ def evaluate_export(test_dir, frames_dir, flows_dir=None, raft=None, gaps=DEFAUL
     record written to metrics.json, the per-frame and per-pair rows, the paths and host timings."""
     t0 = time.perf_counter()
     gaps = check_gaps(gaps)
-    if int(chunk) < 1:
-        raise ValueError('chunk must be >= 1, got %r' % chunk)
+    chunk = chunk_size(chunk)
     if (flows_dir is None) == (raft is None):
         raise ValueError('give exactly one of flows_dir and raft')
-    chunk = int(chunk)
     out = test_dir if out is None else out
     ex = Export(test_dir)
     files = _frame_files(frames_dir)
@@ -236,8 +217,7 @@ def evaluate_export(test_dir, frames_dir, flows_dir=None, raft=None, gaps=DEFAUL
         raise ValueError('the frame files are %dx%d, the export %dx%d' % (fh, fw, ex.H, ex.W))
     by_gap = select_pairs(len(files), gaps, ex.numbers)
     t_read = time.perf_counter() - t0
-    dev = torch.device('cuda', torch.cuda.current_device() if device is None else device)
-    torch.cuda.set_device(dev)
+    dev = cuda_device(device)
     if isinstance(raft, str):
         from .raft import load_raft
         raft = load_raft(raft, dev)
@@ -391,12 +371,9 @@ def parse_args(argv=None):
     p.add_argument('--raft_iters', type=int, default=20, help='RAFT update iterations (as prepare_pairs)')
     p.add_argument('--gaps', type=parse_gaps, default=list(DEFAULT_GAPS), help='frame gaps of the pairs (default 1,2,4,8)')
     p.add_argument('--out', default=None, help='output directory (default: --test_dir)')
-    p.add_argument('--chunk', type=int, default=16, help='frames (pairs) per device copy')
+    p.add_argument('--chunk', type=chunk_size, default=16, help='frames (pairs) per device copy')
     p.add_argument('--gpu', type=int, default=0)
-    a = p.parse_args(argv)
-    if a.chunk < 1:
-        p.error('--chunk must be >= 1')
-    return a
+    return p.parse_args(argv)
 
 
 def main(argv=None):

@@ -3,12 +3,12 @@
 [--chunk 16] [--gpu 0]`.
 
 Reads `depth`, `img_1` and, when the files hold it, `depth_nn` (the per-frame initialisation) of the `batch%04d.npz` files with
-`export_points`' reader (same `--frames`), and blurs every selected frame by each pixel's distance, in disparity, from the
-frame's focal plane. With the refined depth the focus holds still; with the initial depth it boils and hunts, so the two side
-by side show what consistent depth is for. It writes DIR/dof_%05d.png (the refined-depth render, numbered like
-`export_points`' per-frame files), DIR/dof.mp4, DIR/compare.mp4 (frame | initial-depth render | refined-depth render, 30 fps,
-`mp4v`; only when `depth_nn` exists) and DIR/refocus.json (the options, the median depths, each frame's focal disparity and
-mean blur radius for both sources, and whether the comparison was written).
+export_io.Frames (`--frames` as in `export_points`), and blurs every selected frame by each pixel's distance, in
+disparity, from the frame's focal plane. With the refined depth the focus holds still; with the initial depth it boils and
+hunts, so the two side by side show what consistent depth is for. It writes DIR/dof_%05d.png (the refined-depth render,
+numbered like `export_points`' per-frame files), DIR/dof.mp4, DIR/compare.mp4 (frame | initial-depth render | refined-depth
+render, 30 fps, `mp4v`; only when `depth_nn` exists) and DIR/refocus.json (the options, the median depths, each frame's
+focal disparity and mean blur radius for both sources, and whether the comparison was written).
 
 Each depth source is rendered from its own depths. m is the median valid (finite, > 1e-2) depth of its selected frames; the
 blur radius of a pixel is c = min(R, s |disp - phi_t|) pixels, disp = 1/d (0 for an invalid pixel: infinitely far),
@@ -26,45 +26,18 @@ The gather rule (csrc/refocus.cu, include/dvd_b200.h) is exact: the frames are b
 import argparse
 import json
 import os
-import re
 import time
-from concurrent.futures import ThreadPoolExecutor
 
-import cv2
 import numpy as np
 import torch
 
 from . import ops
 from ._lib import DVD_REFOCUS_MAX_RADIUS as MAX_BLUR
-from .export_points import Frames, list_files
+from .export_io import Frames, Writer, chunk_size, cuda_device, frame_range, list_files, to_device
 from .render_views import median_depth
-from .test_videos import _Video
 
 FPS = 30
 F32 = np.float32
-
-
-def read_depth_nn(fr):
-    """The `depth_nn` of the selected frames of `fr` (an export_points.Frames) as [N,H,W] fp32, or None when no file holds
-    it; ValueError when only some do, or when its shape differs from the refined depth's."""
-    have, parts = [], []
-    for f in fr.files:
-        z = np.load(f)
-        have.append('depth_nn' in z.files)
-        if have[-1]:
-            d = np.asarray(z['depth_nn'], dtype=F32)
-            if d.ndim != 4 or d.shape[1] != 1 or d.shape[2:] != (fr.H, fr.W):
-                raise ValueError('%s: depth_nn must be [B,1,%d,%d], got %s' % (f, fr.H, fr.W, d.shape))
-            parts.append(d[:, 0])
-    if not any(have):
-        return None
-    if not all(have):
-        raise ValueError('depth_nn is in %d of the %d files of %s; it must be in all or none'
-                         % (sum(have), len(have), os.path.dirname(fr.files[0])))
-    nn = np.concatenate(parts)
-    if nn.shape[0] != len(fr.where):
-        raise ValueError('depth_nn holds %d frames, depth %d' % (nn.shape[0], len(fr.where)))
-    return np.ascontiguousarray(nn[fr.ids])
 
 
 def source_median(depth, name):
@@ -124,8 +97,7 @@ def check_options(aperture, max_blur, focus_point, focus_window, focus_depth, fo
         raise ValueError('focus_depth must be finite and > 0, got %r' % focus_depth)
     if focus_pull is not None and (len(focus_pull) != 2 or not all(np.isfinite(v) and v > 0 for v in focus_pull)):
         raise ValueError('focus_pull must be two finite values > 0, got %r' % (focus_pull,))
-    if int(chunk) < 1:
-        raise ValueError('chunk must be >= 1, got %r' % chunk)
+    chunk_size(chunk)
 
 
 def refocus(test_dir, out, aperture=8.0, max_blur=16, focus_point=None, focus_window=2, focus_depth=None, focus_pull=None,
@@ -135,12 +107,12 @@ def refocus(test_dir, out, aperture=8.0, max_blur=16, focus_point=None, focus_wi
     the frame numbers and the record written to refocus.json."""
     check_options(aperture, max_blur, focus_point, focus_window, focus_depth, focus_pull, chunk)
     R, chunk = int(max_blur), int(chunk)
-    fr = Frames(list_files(test_dir), frames)
-    N, H, W = fr.N, fr.H, fr.W
-    nn = read_depth_nn(fr)
+    ex = Frames(list_files(test_dir), frames, optional=('depth_nn',))
+    N, H, W = ex.N, ex.H, ex.W
+    nn = ex.depth_nn
     if focus_depth is None and focus_pull is None:
         focus_point = (W // 2, H // 2) if focus_point is None else tuple(int(v) for v in focus_point)
-    sources = [('refined', fr.depth)] + ([('initial', nn)] if nn is not None else [])
+    sources = [('refined', ex.depth)] + ([('initial', nn)] if nn is not None else [])
     med, phi, scale = {}, {}, {}
     for name, d in sources:
         med[name] = source_median(d, '%s depth' % name)
@@ -148,62 +120,47 @@ def refocus(test_dir, out, aperture=8.0, max_blur=16, focus_point=None, focus_wi
         scale[name] = float(F32(float(aperture) * med[name]))
     order = (['initial'] if nn is not None else []) + ['refined']       # the order of the renders in a chunk's buffer
     depth_of = dict(sources)
-    dev = torch.device('cuda', torch.cuda.current_device() if device is None else device)
-    torch.cuda.set_device(dev)
+    dev = cuda_device(device)
 
     os.makedirs(out, exist_ok=True)
-    HW = H * W
     mean_c = {name: np.zeros(N) for name, _ in sources}
     written = []
-    pool = ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1))
-    futures = []
     vids = {'dof': os.path.join(out, 'dof.mp4')}
     if nn is not None:
         vids['compare'] = os.path.join(out, 'compare.mp4')
-    try:
-        v_dof = _Video(vids['dof'], FPS, (H, W))
-        v_cmp = _Video(vids['compare'], FPS, (H, 3 * W)) if nn is not None else None
+    with Writer() as wr:
+        v_dof = wr.video(vids['dof'], FPS, (H, W))
+        v_cmp = wr.video(vids['compare'], FPS, (H, 3 * W)) if nn is not None else None
         for s in range(0, N, chunk):
             e = min(s + chunk, N)
             n = e - s
-            g = torch.from_numpy(np.concatenate([depth_of[name][s:e].reshape(-1) for name in order] + [fr.images(s, e).reshape(-1)] +
-                                                [phi[name][s:e] for name in order])).to(dev)   # the chunk's one H2D copy
-            img = g[len(order) * n * HW:(len(order) + 3) * n * HW].view(n, 3, H, W)
-            fphi = g[(len(order) + 3) * n * HW:]
+            g = to_device(dev, *[depth_of[name][s:e] for name in order], ex.images(s, e), *[phi[name][s:e] for name in order])
+            depths, img, fphi = g[:len(order)], g[len(order)], g[len(order) + 1:]
             # the frame itself (floor(255 clip(img)): no blur) when a comparison is written, then the renders in `order`
             k = len(order) + (nn is not None)
             buf = torch.empty(k, n, H, W, 3, dtype=torch.uint8, device=dev)
             if nn is not None:
-                ops.refocus(g[:n * HW].view(n, H, W), img, fphi[:n], 0.0, 0, out=buf[0])
+                ops.refocus(depths[0], img, fphi[0], 0.0, 0, out=buf[0])
             for j, name in enumerate(order):
-                ops.refocus(g[j * n * HW:(j + 1) * n * HW].view(n, H, W), img, fphi[j * n:(j + 1) * n], scale[name], R,
-                            out=buf[k - len(order) + j])
+                ops.refocus(depths[j], img, fphi[j], scale[name], R, out=buf[k - len(order) + j])
             for name, d in sources:
                 mean_c[name][s:e] = mean_blur(d[s:e], phi[name][s:e], scale[name], R)
             hb = buf.cpu().numpy()                                                       # the chunk's one D2H copy
             for j in range(n):
-                p = os.path.join(out, 'dof_%05d.png' % fr.ids[s + j])
+                p = os.path.join(out, 'dof_%05d.png' % ex.ids[s + j])
                 written.append(p)
-                futures.append(pool.submit(cv2.imwrite, p, hb[-1, j]))
+                wr.png(p, hb[-1, j])
                 v_dof.write(hb[-1, j])
                 if v_cmp is not None:
                     v_cmp.write(np.concatenate(list(hb[:, j]), 1))
-        v_dof.release()
-        if v_cmp is not None:
-            v_cmp.release()
-        for f in futures:
-            if not f.result():
-                raise RuntimeError('cv2.imwrite could not write a frame to %s' % out)
-    finally:
-        pool.shutdown(wait=True)
     options = {'aperture': float(aperture), 'max_blur': R, 'focus_point': None if focus_point is None else list(focus_point),
                'focus_window': int(focus_window), 'focus_depth': focus_depth,
                'focus_pull': None if focus_pull is None else [float(v) for v in focus_pull], 'frames': frames, 'chunk': chunk}
-    rec = record(test_dir, fr.ids, options, H, W, med, scale, phi, mean_c, nn is not None)
+    rec = record(test_dir, ex.ids, options, H, W, med, scale, phi, mean_c, nn is not None)
     with open(os.path.join(out, 'refocus.json'), 'w') as f:
         json.dump(rec, f, indent=1)
     return {'frames_written': written, 'videos': vids, 'json': os.path.join(out, 'refocus.json'),
-            'frames': [int(i) for i in fr.ids], 'record': rec}
+            'frames': [int(i) for i in ex.ids], 'record': rec}
 
 
 def record(test_dir, ids, options, H, W, med, scale, phi, mean_c, compare):
@@ -245,7 +202,7 @@ def parse_args(argv=None):
     g.add_argument('--focus_pull', type=_pair(':', float), default=None, metavar='A:B',
                    help='rack focus from A x to B x the median valid depth, linear in disparity')
     p.add_argument('--focus_window', type=int, default=2, help='--focus_point window half-width k: (2k+1)^2 pixels')
-    p.add_argument('--frames', default=None, help='frames a:b (Python slice of the frames in file order)')
+    p.add_argument('--frames', type=frame_range, default=None, help='frames a:b (Python slice of the frames in file order)')
     p.add_argument('--chunk', type=int, default=16, help='frames per device chunk')
     p.add_argument('--gpu', type=int, default=0)
     a = p.parse_args(argv)
@@ -253,8 +210,6 @@ def parse_args(argv=None):
         check_options(a.aperture, a.max_blur, a.focus_point, a.focus_window, a.focus_depth, a.focus_pull, a.chunk)
     except ValueError as e:
         p.error(str(e))
-    if a.frames is not None and not re.fullmatch(r'-?\d*:-?\d*', a.frames):
-        p.error('--frames must look like a:b, got %r' % a.frames)
     return a
 
 

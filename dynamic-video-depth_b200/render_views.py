@@ -2,9 +2,9 @@
 [--path lock|wiggle] [--ref_frame K] [--amplitude 0.03] [--period 60] [--cameras FILE.npy] [--static auto|none|FILE.ply]
 [--voxel V] [--min_views 2] [--edge_tol 0.05] [--splat 1] [--frames a:b] [--chunk 16] [--gpu 0]`.
 
-Reads `depth`, `img_1`, `K` and `cam_c2w` of the `batch%04d.npz` files as `export_points` does (same reader, same `--frames`,
-`--voxel`, `--edge_tol` and `--min_views`) and renders every selected frame t from a virtual camera. Output frame t shows the
-kept pixels of frame t (`ops.points_select`: finite depth > 1e-2, no flying pixel; colour floor(255 clip(img))) and, unless
+Reads `depth`, `img_1`, `K` and `cam_c2w` of the `batch%04d.npz` files as `export_points` does (export_io.Frames, same
+`--frames`, `--voxel`, `--edge_tol` and `--min_views`) and renders every selected frame t from a virtual camera. Output frame
+t shows the kept pixels of frame t (`ops.points_select`: finite depth > 1e-2, no flying pixel; colour floor(255 clip(img))) and, unless
 `--static none`, the fused static cloud: `auto` fuses it from the selected frames with `points.Fuser` (positions rounded to
 fp32, colours through `points.mean_rgb_to_u8`, what `export_points` writes), a PLY file is read as `export_points` wrote it.
 Moving objects therefore appear only in their own frame; the static cloud fills the background they and the camera motion
@@ -32,17 +32,13 @@ chunk x H x W x 8 bytes: 16 frames of 384 x 224 take 11 MB, which stays in the H
 import argparse
 import json
 import os
-import re
 import time
-from concurrent.futures import ThreadPoolExecutor
 
-import cv2
 import numpy as np
 import torch
 
 from . import ops, points
-from .export_points import Frames, list_files
-from .test_videos import _Video
+from .export_io import Frames, Writer, chunk_size, cuda_device, frame_range, list_files, to_device
 
 PATHS = ('lock', 'wiggle')
 FPS = 30
@@ -141,8 +137,7 @@ def render_views(test_dir, out, path='lock', ref_frame=None, amplitude=0.03, per
     per-view coverage counts and the record written to render.json."""
     if not 1 <= int(splat) <= SPLAT_MAX:
         raise ValueError('splat must be in [1, %d], got %r' % (SPLAT_MAX, splat))
-    if int(chunk) < 1:
-        raise ValueError('chunk must be >= 1, got %r' % chunk)
+    chunk_size(chunk)
     if not edge_tol >= 0:
         raise ValueError('edge_tol must be >= 0, got %r' % edge_tol)
     if int(min_views) < 1:
@@ -150,8 +145,8 @@ def render_views(test_dir, out, path='lock', ref_frame=None, amplitude=0.03, per
     if voxel is not None and not (voxel > 0 and np.isfinite(voxel)):
         raise ValueError('voxel must be positive, got %r' % voxel)
     splat, chunk = int(splat), int(chunk)
-    fr = Frames(list_files(test_dir), frames)
-    N, H, W = fr.N, fr.H, fr.W
+    ex = Frames(list_files(test_dir), frames)
+    N, H, W = ex.N, ex.H, ex.W
     if isinstance(cameras, str):
         cameras = load_cameras(cameras, N)
     elif cameras is not None:
@@ -159,8 +154,8 @@ def render_views(test_dir, out, path='lock', ref_frame=None, amplitude=0.03, per
         if cameras.ndim != 3 or cameras.shape[1:] not in ((3, 4), (4, 4)) or cameras.shape[0] != N:
             raise ValueError('cameras must be [%d,3,4] or [%d,4,4], got %s' % (N, N, cameras.shape))
         cameras = cameras[:, :3]
-    median = median_depth(fr.depth) if cameras is None and path == 'wiggle' else None
-    vK, vc2w = camera_path(fr.K, fr.c2w, fr.ids, path, ref_frame, amplitude, period, median, cameras)
+    median = median_depth(ex.depth) if cameras is None and path == 'wiggle' else None
+    vK, vc2w = camera_path(ex.K, ex.c2w, ex.ids, path, ref_frame, amplitude, period, median, cameras)
     vcams = view_cams(vK, vc2w)
     static_host = None
     if static not in ('auto', 'none'):
@@ -169,22 +164,17 @@ def render_views(test_dir, out, path='lock', ref_frame=None, amplitude=0.03, per
         static_host = points.read_ply(static)
         check_index_range(H, W, static_host[0].shape[0])
     HW = H * W
-    cam30 = points.camera_block(fr.K, fr.c2w)
-    dev = torch.device('cuda', torch.cuda.current_device() if device is None else device)
-    torch.cuda.set_device(dev)
+    cam30 = points.camera_block(ex.K, ex.c2w)
+    dev = cuda_device(device)
 
     def upload(s, e):
         """the chunk's one host-to-device copy: depth [n,H,W], img [n,3,H,W], camera_block [n,30], view cams [n,21]"""
-        n = e - s
-        g = torch.from_numpy(np.concatenate([fr.depth[s:e].reshape(-1), fr.images(s, e).reshape(-1), cam30[s:e].reshape(-1),
-                                             vcams[s:e].reshape(-1)])).to(dev)
-        return (g[:n * HW].view(n, H, W), g[n * HW:4 * n * HW].view(n, 3, H, W), g[4 * n * HW:4 * n * HW + 30 * n].view(n, 30),
-                g[4 * n * HW + 30 * n:].view(n, 21))
+        return to_device(dev, ex.depth[s:e], ex.images(s, e), cam30[s:e], vcams[s:e])
 
     sxyz = srgb = None
     if static == 'auto':
-        vox = voxel if voxel is not None else points.default_voxel(fr.depth)
-        fz = points.Fuser(H, W, vox, points.default_origin(fr.c2w, vox), edge_tol, min_views)
+        vox = voxel if voxel is not None else points.default_voxel(ex.depth)
+        fz = points.Fuser(H, W, vox, points.default_origin(ex.c2w, vox), edge_tol, min_views)
         for s in range(0, N, chunk):
             depth, img, cam, _ = upload(s, min(s + chunk, N))
             fz.add(depth, img, cam)
@@ -202,11 +192,9 @@ def render_views(test_dir, out, path='lock', ref_frame=None, amplitude=0.03, per
     rgb_tmpl = torch.zeros(H, W, 3, dtype=torch.uint8, device=dev)
     coverage = np.zeros(N, dtype=np.int64)
     written = []
-    pool = ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1))
-    futures = []
     vids = {'views': os.path.join(out, 'views.mp4'), 'compare': os.path.join(out, 'compare.mp4')}
-    try:
-        v_views, v_cmp = _Video(vids['views'], FPS, (H, W)), _Video(vids['compare'], FPS, (H, 2 * W))
+    with Writer() as wr:
+        v_views, v_cmp = wr.video(vids['views'], FPS, (H, W)), wr.video(vids['compare'], FPS, (H, 2 * W))
         for s in range(0, N, chunk):
             e = min(s + chunk, N)
             n = e - s
@@ -226,26 +214,20 @@ def render_views(test_dir, out, path='lock', ref_frame=None, amplitude=0.03, per
             views_h = hb[4 * n:4 * n + n * HW * 3].reshape(n, H, W, 3)
             orig_h = hb[4 * n + n * HW * 3:].reshape(n, H, W, 3)
             for j in range(n):
-                p = os.path.join(out, 'view_%05d.png' % fr.ids[s + j])
+                p = os.path.join(out, 'view_%05d.png' % ex.ids[s + j])
                 written.append(p)
-                futures.append(pool.submit(cv2.imwrite, p, views_h[j]))
+                wr.png(p, views_h[j])
                 v_views.write(views_h[j])
                 v_cmp.write(np.concatenate([orig_h[j], views_h[j]], 1))
-        v_views.release(), v_cmp.release()
-        for f in futures:
-            if not f.result():
-                raise RuntimeError('cv2.imwrite could not write a view to %s' % out)
-    finally:
-        pool.shutdown(wait=True)
     options = {'path': 'cameras' if cameras is not None else path, 'ref_frame': ref_frame, 'amplitude': amplitude,
                'period': period, 'median_depth': median, 'static': static, 'voxel': voxel, 'min_views': min_views,
                'edge_tol': edge_tol, 'splat': splat, 'frames': frames, 'chunk': chunk}
     if path == 'lock' and cameras is None:
-        options['ref_frame'] = int(fr.ids[N // 2]) if ref_frame is None else int(ref_frame)
-    rec = record(test_dir, fr.ids, vK, vc2w, coverage, options, H, W, n_static)
+        options['ref_frame'] = int(ex.ids[N // 2]) if ref_frame is None else int(ref_frame)
+    rec = record(test_dir, ex.ids, vK, vc2w, coverage, options, H, W, n_static)
     with open(os.path.join(out, 'render.json'), 'w') as f:
         json.dump(rec, f, indent=1)
-    return {'views': written, 'videos': vids, 'json': os.path.join(out, 'render.json'), 'frames': [int(i) for i in fr.ids],
+    return {'views': written, 'videos': vids, 'json': os.path.join(out, 'render.json'), 'frames': [int(i) for i in ex.ids],
             'coverage': coverage, 'record': rec}
 
 
@@ -269,13 +251,10 @@ def parse_args(argv=None):
     p.add_argument('--edge_tol', type=float, default=points.EDGE_TOL,
                    help='drop a pixel when |d - d_n| / d exceeds this for one of its 4-neighbours (flying pixels)')
     p.add_argument('--splat', type=int, default=1, help='footprint of a point: splat x splat pixels (1 to %d)' % SPLAT_MAX)
-    p.add_argument('--frames', default=None, help='frames a:b (Python slice of the frames in file order)')
+    p.add_argument('--frames', type=frame_range, default=None, help='frames a:b (Python slice of the frames in file order)')
     p.add_argument('--chunk', type=int, default=16, help='frames per device chunk')
     p.add_argument('--gpu', type=int, default=0)
-    a = p.parse_args(argv)
-    if a.frames is not None and not re.fullmatch(r'-?\d*:-?\d*', a.frames):
-        p.error('--frames must look like a:b, got %r' % a.frames)
-    return a
+    return p.parse_args(argv)
 
 
 def main(argv=None):

@@ -2,8 +2,9 @@
 `python -m dvd_b200.test_videos --test_dir OUT/<net>_<dataset>_<suffix>/epochbest_test [--slice_rows a:b] [--chunk 32]
 [--gpu 0]`, or `python -m dvd_b200.test --videos …` after the export.
 
-Reads `depth`, `depth_nn`, `depth_gt` and `img_1` of the `batch%04d.npz` files (in index order, flattened) and writes, with
-the reference's names (`outdir` = the `epoch*_test` directory, `parent` its parent, `epoch_string` its name):
+Reads `depth`, `depth_nn`, `depth_gt` and `img_1` of the `batch%04d.npz` files with export_io.Frames (in index order,
+flattened) and writes, with the reference's names (`outdir` = the `epoch*_test` directory, `parent` its parent,
+`epoch_string` its name):
 
 * `outdir/compare_%04d.png`: refined, initial (MiDaS) and GT disparity in the turbo colour map, all three over the range of
   the refined disparity of the whole video: vmin = 1 / max(depth), vmax = 1 / min(depth), fp32;
@@ -44,14 +45,13 @@ import html
 import os
 import re
 import time
-from concurrent.futures import ThreadPoolExecutor
 
 import cv2
 import numpy as np
 import torch
 
 from . import ops
-from .export_points import list_files
+from .export_io import Frames, Writer, chunk_size, cuda_device, list_files, to_device
 
 KEYS = ('depth', 'depth_nn', 'depth_gt', 'img_1')
 MARGIN, TITLE_H, BAR_GAP, BAR_W, LABEL_GAP, LABEL_W, BAR_MIN_H = 8, 32, 6, 14, 4, 72, 48
@@ -112,50 +112,6 @@ def slice_rows_for(H, rows=None):
     return a, b
 
 
-def read_export(files):
-    """The four arrays of the files, flattened in file order: depth, depth_nn, depth_gt [N,1,H,W], img_1 [N,3,H,W] fp32, and the
-    file of each frame."""
-    arrs, where = {k: [] for k in KEYS}, []
-    for f in files:
-        z = np.load(f)
-        missing = [k for k in KEYS if k not in z.files]
-        if missing:
-            raise ValueError('%s lacks %s' % (f, ', '.join(missing)))
-        a = {k: np.asarray(z[k], dtype=np.float32) for k in KEYS}
-        d = a['depth']
-        if d.ndim != 4 or d.shape[1] != 1:
-            raise ValueError('%s: depth must be [B,1,H,W], got %s' % (f, d.shape))
-        B, _, H, W = d.shape
-        for k, shape in (('depth_nn', d.shape), ('depth_gt', d.shape), ('img_1', (B, 3, H, W))):
-            if a[k].shape != shape:
-                raise ValueError('%s: %s %s does not match depth %s' % (f, k, a[k].shape, d.shape))
-        if arrs['depth'] and d.shape[2:] != arrs['depth'][0].shape[2:]:
-            raise ValueError('%s: frames of %dx%d, the first file has %dx%d' % (f, H, W, *arrs['depth'][0].shape[2:]))
-        for k in KEYS:
-            arrs[k].append(a[k])
-        where += [f] * B
-    return {k: np.concatenate(v) for k, v in arrs.items()}, where
-
-
-def _even(img):
-    h, w = img.shape[:2]
-    return np.pad(img, ((0, h % 2), (0, w % 2), (0, 0))) if h % 2 or w % 2 else img
-
-
-class _Video:
-    def __init__(self, path, fps, shape):
-        h, w = shape[0] + shape[0] % 2, shape[1] + shape[1] % 2
-        self.w = cv2.VideoWriter(path, cv2.VideoWriter_fourcc(*'mp4v'), fps, (w, h))
-        if not self.w.isOpened():
-            raise RuntimeError('cv2.VideoWriter could not open %s (mp4v, %dx%d)' % (path, w, h))
-
-    def write(self, frame):
-        self.w.write(_even(frame))
-
-    def release(self):
-        self.w.release()
-
-
 def _page(epoch_string, loss, rows):
     videos = (('%s_rgb.mp4' % epoch_string, 'original video'),
               ('%s.mp4' % epoch_string, 'Disparity loss %.6g' % loss),
@@ -169,23 +125,21 @@ def render_test_videos(test_dir, slice_rows=None, chunk=32, device=None):
     """Writes the frames, slices, videos and page of the test export in `test_dir` (see the module docstring) on CUDA device
     `device` (default: the current one). The files are read and checked before the device is touched. Returns a dict of the
     written paths, the frame count, the slice rows and the page's loss."""
-    if chunk < 1:
-        raise ValueError('chunk must be >= 1, got %d' % chunk)
+    chunk = chunk_size(chunk)
     outdir = os.path.normpath(test_dir)
     parent, epoch_string = os.path.dirname(outdir), os.path.basename(outdir)
-    ex, where = read_export(list_files(outdir))
-    N, _, H, W = ex['depth'].shape
+    ex = Frames(list_files(outdir), keys=KEYS)
+    N, H, W = ex.N, ex.H, ex.W
     a, b = slice_rows_for(H, slice_rows)
-    bad = ~(np.isfinite(ex['depth']) & (ex['depth'] > 0)).reshape(N, -1).all(1)
+    bad = ~(np.isfinite(ex.depth) & (ex.depth > 0)).reshape(N, -1).all(1)
     if bad.any():
         i = int(np.argmax(bad))
-        raise ValueError('frame %d (%s) has a refined depth that is not finite and > 0' % (i, where[i]))
-    dev = torch.device('cuda', torch.cuda.current_device() if device is None else device)
-    torch.cuda.set_device(dev)
+        raise ValueError('frame %d (%s) has a refined depth that is not finite and > 0' % (i, ex.file_of[i]))
+    dev = cuda_device(device)
     lut_h = turbo_lut()
     lut = torch.from_numpy(lut_h).to(dev)
-    dd = torch.from_numpy(np.stack([ex['depth'], ex['depth_nn']])).to(dev)     # both stay on the device for the whole run
-    depth, depth_nn = dd[0], dd[1]
+    # both stay on the device for the whole run
+    depth, depth_nn = to_device(dev, ex.depth[:, None], ex.depth_nn[:, None])
     # the global range: vmin = 1 / max, vmax = 1 / min in fp32 (numpy 2: a Python int over a float32 scalar stays float32)
     rng = torch.stack([1 / depth.amax(), 1 / depth.amin()])
     host = rng.cpu().numpy()
@@ -198,23 +152,19 @@ def render_test_videos(test_dir, slice_rows=None, chunk=32, device=None):
     sse = torch.empty(N, dtype=torch.float32, device=dev)
     ncmp, nrgb = CH * CW * 3, HW * 3
     written = {'compare': [], 'rgb': [], 'temporal_slice': []}
-    pool = ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1))
-    futures = []
-
-    def png(kind, i, img):
-        path = os.path.join(outdir, '%s_%04d.png' % (kind, i))
-        written[kind].append(path)
-        futures.append(pool.submit(cv2.imwrite, path, img))
-
     vids = {'compare': os.path.join(parent, epoch_string + '.mp4'), 'rgb': os.path.join(parent, epoch_string + '_rgb.mp4'),
             'temporal': os.path.join(parent, epoch_string + '_temporal.mp4')}
-    try:
-        v_cmp, v_rgb = _Video(vids['compare'], FPS, (CH, CW)), _Video(vids['rgb'], FPS, (H, W))
+    with Writer() as out:
+        def png(kind, i, img):
+            path = os.path.join(outdir, '%s_%04d.png' % (kind, i))
+            written[kind].append(path)
+            out.png(path, img)
+
+        v_cmp, v_rgb = out.video(vids['compare'], FPS, (CH, CW)), out.video(vids['rgb'], FPS, (H, W))
         for s in range(0, N, chunk):
             e = min(s + chunk, N)
             n = e - s
-            up = torch.from_numpy(np.concatenate([ex['depth_gt'][s:e].reshape(-1), ex['img_1'][s:e].reshape(-1)])).to(dev)
-            gt, img = up[:n * HW].view(n, 1, H, W), up[n * HW:].view(n, 3, H, W)
+            gt, img = to_device(dev, ex.depth_gt[s:e, None], ex.images(s, e))
             ops.disp_vali(depth[s:e], gt, out=sse[s:e])
             buf = torch.empty(n * (ncmp + nrgb), dtype=torch.uint8, device=dev)
             cmp_out, rgb_out = buf[:n * ncmp].view(n, CH, CW, 3), buf[n * ncmp:].view(n, H, W, 3)
@@ -229,7 +179,6 @@ def render_test_videos(test_dir, slice_rows=None, chunk=32, device=None):
                 png('rgb', s + j, rgb_h[j])
                 v_cmp.write(cmp_h[j])
                 v_rgb.write(rgb_h[j])
-        v_cmp.release(), v_rgb.release()
 
         # temporal slices: panel row = frame, read in place from the resident depth maps; ranges per slice and panel on the device
         S = b - a
@@ -248,16 +197,10 @@ def render_test_videos(test_dir, slice_rows=None, chunk=32, device=None):
                   for p, (src, (y0, x0)) in enumerate(zip((depth, depth_nn), spos))]
         ops.vis_panels(stmpl, panels, lut, sl, tmpl_stride=sCH * sCW * 3)
         sl_h = sl.cpu().numpy()
-        v_sl = _Video(vids['temporal'], FPS_SLICES, (sCH, sCW))
+        v_sl = out.video(vids['temporal'], FPS_SLICES, (sCH, sCW))
         for r in range(S):
             png('temporal_slice', r, sl_h[r])
             v_sl.write(sl_h[r])
-        v_sl.release()
-        for f in futures:
-            if not f.result():
-                raise RuntimeError('cv2.imwrite could not write a frame to %s' % outdir)
-    finally:
-        pool.shutdown(wait=True)
     loss = float((sse.double() / HW).mean())
     page = os.path.join(parent, epoch_string + '.html')
     with open(page, 'w') as f:
@@ -270,11 +213,9 @@ def parse_args(argv=None):
     p.add_argument('--test_dir', required=True, help='the epoch*_test directory of batch%%04d.npz files the test driver wrote')
     p.add_argument('--slice_rows', default=None,
                    help='image rows a:b of the temporal slices (default 120:140, or the middle 20 rows when H < 140)')
-    p.add_argument('--chunk', type=int, default=32, help='frames per device chunk')
+    p.add_argument('--chunk', type=chunk_size, default=32, help='frames per device chunk')
     p.add_argument('--gpu', type=int, default=0)
     a = p.parse_args(argv)
-    if a.chunk < 1:
-        p.error('--chunk must be >= 1')
     if a.slice_rows is not None and not re.fullmatch(r'\d+:\d+', a.slice_rows):
         p.error('--slice_rows must look like a:b, got %r' % a.slice_rows)
     return a

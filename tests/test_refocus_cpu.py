@@ -191,17 +191,16 @@ def _export(d, N, H, W, nn=True, per_file=2, nn_files=None):
     return str(d), depth[:, 0]
 
 
-def test_depth_nn_reader(tmp_path):
-    from dvd_b200 import refocus as rf
-    from dvd_b200.export_points import Frames, list_files
+def test_depth_nn_is_read_with_the_frames(tmp_path):
+    from dvd_b200.export_io import Frames, list_files
     d, depth = _export(tmp_path / 'a', 5, 6, 7)
-    nn = rf.read_depth_nn(Frames(list_files(d), '1:4'))
+    nn = Frames(list_files(d), '1:4', optional=('depth_nn',)).depth_nn
     assert np.array_equal(nn, depth[1:4] * F32(1.5))
     d, _ = _export(tmp_path / 'b', 5, 6, 7, nn=False)
-    assert rf.read_depth_nn(Frames(list_files(d))) is None
+    assert Frames(list_files(d), optional=('depth_nn',)).depth_nn is None
     d, _ = _export(tmp_path / 'c', 5, 6, 7, nn_files=(0, 2))
-    with pytest.raises(ValueError):
-        rf.read_depth_nn(Frames(list_files(d)))
+    with pytest.raises(ValueError, match='depth_nn'):
+        Frames(list_files(d), optional=('depth_nn',))
 
 
 def test_errors_once_the_files_are_read(tmp_path):

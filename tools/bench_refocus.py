@@ -21,9 +21,7 @@ import subprocess
 import sys
 import tempfile
 import time
-from concurrent.futures import ThreadPoolExecutor
 
-import cv2
 import numpy as np
 import torch
 
@@ -84,30 +82,29 @@ def device_pass(chunks, scales, R):
 
 def run(N, H, W, radii, oracle_frames, workdir):
     from dvd_b200 import refocus as rf
-    from dvd_b200.export_points import Frames, list_files
-    from dvd_b200.test_videos import _Video
+    from dvd_b200.export_io import Frames, Writer, list_files
     from oracle import refocus as orf
     d = os.path.join(workdir, 'exp_%dx%dx%d' % (N, H, W))
     os.makedirs(d)
     synth_export(d, N, H, W)
     dev = torch.device('cuda')
-    fr = Frames(list_files(d))
-    nn = rf.read_depth_nn(fr)
-    m, m_nn = rf.source_median(fr.depth, 'refined'), rf.source_median(nn, 'initial')
-    phi, phi_nn = rf.focus_disparities(fr.depth, m, focus_pull=PULL), rf.focus_disparities(nn, m_nn, focus_pull=PULL)
+    ex = Frames(list_files(d), optional=('depth_nn',))
+    depth, nn = ex.depth, ex.depth_nn
+    m, m_nn = rf.source_median(depth, 'refined'), rf.source_median(nn, 'initial')
+    phi, phi_nn = rf.focus_disparities(depth, m, focus_pull=PULL), rf.focus_disparities(nn, m_nn, focus_pull=PULL)
     scales = {'refined': float(F32(APERTURE * m)), 'initial': float(F32(APERTURE * m_nn))}
     chunks = []
     for s in range(0, N, CHUNK):
         e = min(s + CHUNK, N)
         chunks.append(tuple(torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-                            for a in (fr.depth[s:e], nn[s:e], fr.images(s, e), phi[s:e], phi_nn[s:e])))
+                            for a in (depth[s:e], nn[s:e], ex.images(s, e), phi[s:e], phi_nn[s:e])))
     out = {'frames': N, 'H': H, 'W': W, 'median_depth': m, 'radii': {}}
     for R in radii:
         device_pass(chunks, scales, R)                                                  # warm-up
         best = min((device_pass(chunks, scales, R) for _ in range(3)), key=lambda r: r[0])
         ms_ref, ms_all, outs = best
         taps = rule_taps(H, W, R) * N
-        mean_c = float(np.mean(rf.mean_blur(fr.depth, phi, scales['refined'], R)))
+        mean_c = float(np.mean(rf.mean_blur(depth, phi, scales['refined'], R)))
         t0 = time.perf_counter()
         host = [b.cpu().numpy() for b in outs]
         d2h = time.perf_counter() - t0
@@ -116,15 +113,16 @@ def run(N, H, W, radii, oracle_frames, workdir):
         o = os.path.join(workdir, 'out_%dx%dx%d_%d' % (N, H, W, R))
         os.makedirs(o)
         t0 = time.perf_counter()
-        with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as pool:
-            assert all(pool.map(lambda j: cv2.imwrite(os.path.join(o, 'dof_%05d.png' % j), frames[j]), range(N)))
+        with Writer() as w:
+            for j in range(N):
+                w.png(os.path.join(o, 'dof_%05d.png' % j), frames[j])
         png = time.perf_counter() - t0
         t0 = time.perf_counter()
-        v1, v2 = _Video(os.path.join(o, 'dof.mp4'), 30, (H, W)), _Video(os.path.join(o, 'compare.mp4'), 30, (H, 3 * W))
-        for j in range(N):
-            v1.write(frames[j])
-            v2.write(cmp[j])
-        v1.release(), v2.release()
+        with Writer() as w:
+            v1, v2 = w.video(os.path.join(o, 'dof.mp4'), 30, (H, W)), w.video(os.path.join(o, 'compare.mp4'), 30, (H, 3 * W))
+            for j in range(N):
+                v1.write(frames[j])
+                v2.write(cmp[j])
         mp4 = time.perf_counter() - t0
         t0 = time.perf_counter()
         rf.refocus(d, os.path.join(workdir, 'cli_%dx%dx%d_%d' % (N, H, W, R)), aperture=APERTURE, max_blur=R, focus_pull=PULL)
@@ -132,7 +130,7 @@ def run(N, H, W, radii, oracle_frames, workdir):
         whole = time.perf_counter() - t0
         k = min(oracle_frames, N)
         t0 = time.perf_counter()
-        ref = orf.render(fr.depth[:k], fr.images(0, k), phi[:k], F32(scales['refined']), R)
+        ref = orf.render(depth[:k], ex.images(0, k), phi[:k], F32(scales['refined']), R)
         cpu_per_frame = (time.perf_counter() - t0) / k
         out['radii'][R] = {'refined_kernel_ms': ms_ref, 'three_launches_ms': ms_all, 'rule_taps': taps,
                            'rule_taps_per_s': taps / (ms_ref / 1e3), 'mean_blur_radius': mean_c, 'd2h_ms': d2h * 1e3,

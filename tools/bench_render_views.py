@@ -21,9 +21,7 @@ import subprocess
 import sys
 import tempfile
 import time
-from concurrent.futures import ThreadPoolExecutor
 
-import cv2
 import numpy as np
 import torch
 
@@ -69,9 +67,9 @@ class Timer:
         return r
 
 
-def device_pass(chunks, fr, splat, static, sxyz, srgb, vox, origin):
+def device_pass(chunks, ex, splat, static, sxyz, srgb, vox, origin):
     from dvd_b200 import ops, points
-    H, W, HW = fr.H, fr.W, fr.H * fr.W
+    H, W, HW = ex.H, ex.W, ex.H * ex.W
     t = Timer()
     if static:
         def fuse():
@@ -100,13 +98,13 @@ def device_pass(chunks, fr, splat, static, sxyz, srgb, vox, origin):
     return t.ms, n_frame_pts, outs
 
 
-def static_splat_ms(fr, vcams_dev, sxyz, splat, chunk, dev):
+def static_splat_ms(ex, vcams_dev, sxyz, splat, chunk, dev):
     """static splat alone over all frames with a given chunk (key buffers filled outside the timed window)"""
     from dvd_b200 import ops
     ms = 0.0
-    for s in range(0, fr.N, chunk):
-        e = min(s + chunk, fr.N)
-        keys = ops.view_keys(e - s, fr.H, fr.W, dev)
+    for s in range(0, ex.N, chunk):
+        e = min(s + chunk, ex.N)
+        keys = ops.view_keys(e - s, ex.H, ex.W, dev)
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
         ops.splat_views(keys, sxyz, vcams_dev[s:e], splat)
@@ -119,29 +117,22 @@ def static_splat_ms(fr, vcams_dev, sxyz, splat, chunk, dev):
 
 def run(N, H, W, splat, oracle_frames, workdir):
     from dvd_b200 import points, render_views as rv
-    from dvd_b200.export_points import Frames, list_files
-    from dvd_b200.test_videos import _Video
+    from dvd_b200.export_io import Frames, Writer, list_files, to_device
     from oracle import render_views as orv
     d = os.path.join(workdir, 'exp_%dx%dx%d' % (N, H, W))
     os.makedirs(d)
     synth_export(d, N, H, W)
     dev = torch.device('cuda')
-    fr = Frames(list_files(d))
+    ex = Frames(list_files(d))
     HW = H * W
-    vK, vc2w = rv.camera_path(fr.K, fr.c2w, fr.ids, 'wiggle', median=rv.median_depth(fr.depth))
+    vK, vc2w = rv.camera_path(ex.K, ex.c2w, ex.ids, 'wiggle', median=rv.median_depth(ex.depth))
     vcams = rv.view_cams(vK, vc2w)
-    cam30 = points.camera_block(fr.K, fr.c2w)
+    cam30 = points.camera_block(ex.K, ex.c2w)
     chunk = 16
-    chunks = []
-    for s in range(0, N, chunk):
-        e = min(s + chunk, N)
-        n = e - s
-        g = torch.from_numpy(np.concatenate([fr.depth[s:e].reshape(-1), fr.images(s, e).reshape(-1), cam30[s:e].reshape(-1),
-                                             vcams[s:e].reshape(-1)])).to(dev)
-        chunks.append((g[:n * HW].view(n, H, W), g[n * HW:4 * n * HW].view(n, 3, H, W), g[4 * n * HW:4 * n * HW + 30 * n].view(n, 30),
-                       g[4 * n * HW + 30 * n:].view(n, 21)))
-    vox = points.default_voxel(fr.depth)
-    origin = points.default_origin(fr.c2w, vox)
+    chunks = [to_device(dev, ex.depth[s:s + chunk], ex.images(s, min(s + chunk, N)), cam30[s:s + chunk],
+                        vcams[s:s + chunk]) for s in range(0, N, chunk)]
+    vox = points.default_voxel(ex.depth)
+    origin = points.default_origin(ex.c2w, vox)
     fz = points.Fuser(H, W, vox, origin, points.EDGE_TOL, 2)
     for depth, img, cam, _ in chunks:
         fz.add(depth, img, cam)
@@ -151,16 +142,16 @@ def run(N, H, W, splat, oracle_frames, workdir):
     srgb_h = points.mean_rgb_to_u8(res['rgb'].cpu().numpy())
     srgb = torch.from_numpy(srgb_h).to(dev)
     R = sxyz.shape[0]
-    device_pass(chunks, fr, splat, True, sxyz, srgb, vox, origin)                      # warm-up
+    device_pass(chunks, ex, splat, True, sxyz, srgb, vox, origin)                      # warm-up
     best = None
     for _ in range(3):
-        ms, n_frame_pts, outs = device_pass(chunks, fr, splat, True, sxyz, srgb, vox, origin)
+        ms, n_frame_pts, outs = device_pass(chunks, ex, splat, True, sxyz, srgb, vox, origin)
         best = ms if best is None or sum(ms.values()) < sum(best.values()) else best
     vcams_dev = torch.from_numpy(vcams).to(dev)
     residency = {}
     for c in (16, 64, N):
-        static_splat_ms(fr, vcams_dev, sxyz, splat, c, dev)
-        t = min(static_splat_ms(fr, vcams_dev, sxyz, splat, c, dev) for _ in range(3))
+        static_splat_ms(ex, vcams_dev, sxyz, splat, c, dev)
+        t = min(static_splat_ms(ex, vcams_dev, sxyz, splat, c, dev) for _ in range(3))
         residency[c] = {'ms': t, 'key_buffer_MB': min(c, N) * HW * 8 / 1e6, 'pairs_per_s': R * N / (t / 1e3)}
     # host stages: D2H per chunk, PNG, mp4
     t0 = time.perf_counter()
@@ -171,15 +162,16 @@ def run(N, H, W, splat, oracle_frames, workdir):
     out = os.path.join(workdir, 'out_%dx%dx%d' % (N, H, W))
     os.makedirs(out)
     t0 = time.perf_counter()
-    with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as pool:
-        assert all(pool.map(lambda j: cv2.imwrite(os.path.join(out, 'view_%05d.png' % j), views[j]), range(N)))
+    with Writer() as w:
+        for j in range(N):
+            w.png(os.path.join(out, 'view_%05d.png' % j), views[j])
     png = time.perf_counter() - t0
     t0 = time.perf_counter()
-    v1, v2 = _Video(os.path.join(out, 'views.mp4'), 30, (H, W)), _Video(os.path.join(out, 'compare.mp4'), 30, (H, 2 * W))
-    for j in range(N):
-        v1.write(views[j])
-        v2.write(np.concatenate([origs[j], views[j]], 1))
-    v1.release(), v2.release()
+    with Writer() as w:
+        v1, v2 = w.video(os.path.join(out, 'views.mp4'), 30, (H, W)), w.video(os.path.join(out, 'compare.mp4'), 30, (H, 2 * W))
+        for j in range(N):
+            v1.write(views[j])
+            v2.write(np.concatenate([origs[j], views[j]], 1))
     mp4 = time.perf_counter() - t0
     # one whole call of the command's function
     t0 = time.perf_counter()
@@ -190,7 +182,7 @@ def run(N, H, W, splat, oracle_frames, workdir):
     k = min(oracle_frames, N)
     P = points.world_points(chunks[0][0][:k].contiguous(), chunks[0][2][:k].contiguous()).cpu().numpy()
     t0 = time.perf_counter()
-    ref, _ = orv.render(fr.depth[:k], fr.images(0, k), P, vK[:k], vc2w[:k], splat, (sxyz.cpu().numpy(), srgb_h))
+    ref, _ = orv.render(ex.depth[:k], ex.images(0, k), P, vK[:k], vc2w[:k], splat, (sxyz.cpu().numpy(), srgb_h))
     cpu_per_frame = (time.perf_counter() - t0) / k
     equal = bool(np.array_equal(ref, views[:k]))
     splat_ms = best['splat_frame'] + best['splat_static']
