@@ -65,6 +65,7 @@ DVD_VIS_MAX_PANELS = 4
 DVD_VIEW_CAM_FLOATS = 21
 DVD_SPLAT_MAX = 4
 DVD_REFOCUS_MAX_RADIUS = 32
+DVD_TRACK_MAX_TAIL = 64
 
 
 class VisMap(ctypes.Structure):
@@ -187,6 +188,9 @@ SIGNATURES = {
     'dvd_depth_metrics': [_P, _P, _P, _P, _P, _P, _I, _I, _I, _P],
     'dvd_pair_consistency_partials_size': [_I, _I, _I],
     'dvd_pair_consistency': [_P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P],
+    'dvd_pair_consistency_sf_partials_size': [_I, _I, _I],
+    'dvd_pair_consistency_sf': [_P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P],
+    'dvd_draw_tracks': [_P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P],
     'dvd_vis_ranges': [ctypes.POINTER(VisMap), _I, _I, _I, _P, _P],
     'dvd_vis_tiles': [ctypes.POINTER(VisMap), _I, _I, _I, _P, _P, _P, _P, _P],
 }
@@ -198,7 +202,8 @@ _RESTYPES = {'dvd_last_error': ctypes.c_char_p, 'dvd_struct_size': ctypes.c_long
              'dvd_aa_resize_scratch_bytes': ctypes.c_long, 'dvd_points_select_scratch_bytes': ctypes.c_long,
              'dvd_voxel_reduce_scratch_bytes': ctypes.c_long, 'dvd_ordered_workspace_bytes': ctypes.c_size_t,
              'dvd_reproject_ordered_bytes': ctypes.c_size_t, 'dvd_masked_select_partials_size': _L,
-             'dvd_depth_metrics_partials_size': _L, 'dvd_pair_consistency_partials_size': _L}
+             'dvd_depth_metrics_partials_size': _L, 'dvd_pair_consistency_partials_size': _L,
+             'dvd_pair_consistency_sf_partials_size': _L}
 
 # sites of dvd_ordered_workspace_bytes (include/dvd_b200.h)
 DVD_ORD_CONV_WGRAD, DVD_ORD_MLP_WGRAD, DVD_ORD_MLP_DGRAD, DVD_ORD_CHANNEL_SUMS, DVD_ORD_STEM, DVD_ORD_HEAD = range(6)

@@ -14,26 +14,16 @@
 // any order.
 #include <math.h>
 
-#include "common.cuh"
+#include "pair_consistency.cuh"
 
 namespace dvd {
 namespace {
 
-constexpr int kThreads = 256;
-constexpr int kMaxParts = 128;           // blocks per frame (pair) in the partial-sum kernels
-constexpr int kPixelsPerThread = 8;
 constexpr int kSelectPixelsPerThread = 32;
 constexpr int kBins = 256;
 constexpr int kSelectState = 3;          // per segment: key prefix, remaining rank, valid count
 constexpr int kMetricSlots = 2 * 22;     // per source: count, then per scale 7 sums
 constexpr int kPairSlots = 2 * 2 * 6;    // per source and region: count, behind, sum e_r, sum e_d, #e_r < 1, #e_r < 3
-
-int parts_for(long hw, int per_thread) {
-  const long want = (hw + (long)kThreads * per_thread - 1) / ((long)kThreads * per_thread);
-  return (int)(want < 1 ? 1 : (want > kMaxParts ? kMaxParts : want));
-}
-
-__device__ __forceinline__ bool valid_depth(float v) { return isfinite(v) && v > 1e-2f; }
 
 // order-preserving map of fp32 bits to uint32 (negative values flipped, positive ones offset past them), and its inverse
 __device__ __forceinline__ unsigned int order_key(float v) {
@@ -42,40 +32,6 @@ __device__ __forceinline__ unsigned int order_key(float v) {
 }
 __device__ __forceinline__ float key_value(unsigned int k) {
   return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-
-__device__ __forceinline__ double warp_sum_d(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = __dadd_rn(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-
-// acc[K] of every thread -> dst[K] (thread order -> warp xor tree -> warps in index order). red: [kThreads / 32][K] doubles.
-template <int K>
-__device__ __forceinline__ void block_sums(const double (&acc)[K], double* red, double* dst) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-#pragma unroll
-  for (int j = 0; j < K; ++j) {
-    const double v = warp_sum_d(acc[j]);
-    if (lane == 0) red[warp * K + j] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < K) {
-    double s = 0.0;
-    for (int w = 0; w < kThreads / 32; ++w) s = __dadd_rn(s, red[w * K + threadIdx.x]);
-    dst[threadIdx.x] = s;
-  }
-}
-
-// grid (n segments), block K: out[s][j] = sum over p of partials[s][p][j], p ascending
-__global__ void reduce_partials_kernel(const double* __restrict__ partials, double* __restrict__ out, int P, int K) {
-  DVD_PDL_ENTER();
-  const long s = blockIdx.x;
-  const int j = threadIdx.x;
-  if (j >= K) return;
-  double acc = 0.0;
-  for (int p = 0; p < P; ++p) acc = __dadd_rn(acc, partials[(s * P + p) * K + j]);
-  out[s * K + j] = acc;
 }
 
 // ---- masked selection ---------------------------------------------------------------------------------------------------------
@@ -204,12 +160,8 @@ __global__ void __launch_bounds__(kThreads) depth_metrics_partial_kernel(const f
 }
 
 // ---- consistency along the flow -----------------------------------------------------------------------------------------------
-// cam [30] = K^T | (K^-1)^T | R | t (fp32, dvd_b200.points.camera_block): K[r][c] = cam[3 c + r], Kinv[r][c] = cam[9 + 3 c + r],
-// R[r][c] = cam[18 + 3 r + c], t[r] = cam[27 + r]
-__device__ __forceinline__ double dot3(double a0, double a1, double a2, double x, double y, double z) {
-  return __dadd_rn(__dadd_rn(__dmul_rn(a0, x), __dmul_rn(a1, y)), __dmul_rn(a2, z));
-}
-
+// the per-pixel rule is pair_pixel (pair_consistency.cuh); per source, slots 12 src + 6 region + {count, behind, sum e_r, sum e_d,
+// #e_r < 1, #e_r < 3}, regions all and static
 __global__ void __launch_bounds__(kThreads) pair_consistency_partial_kernel(
     const float* __restrict__ depth, const float* __restrict__ depth_nn, const float* __restrict__ cam,
     const int* __restrict__ ia, const int* __restrict__ ib, const float* __restrict__ flow, const unsigned char* __restrict__ mask,
@@ -219,10 +171,7 @@ __global__ void __launch_bounds__(kThreads) pair_consistency_partial_kernel(
   __shared__ double cm[2][30];
   const long pair = blockIdx.y, P = gridDim.x, hw = (long)H * W;
   const long fa = ia[pair], fb = ib[pair];
-  if (threadIdx.x < 60) cm[threadIdx.x / 30][threadIdx.x % 30] = (double)cam[(threadIdx.x < 30 ? fa : fb) * 30 + threadIdx.x % 30];
-  __syncthreads();
-  const double* A = cm[0];
-  const double* B = cm[1];
+  stage_pair_cameras(cam, fa, fb, cm);
   double acc[kPairSlots];
 #pragma unroll
   for (int j = 0; j < kPairSlots; ++j) acc[j] = 0.0;
@@ -230,63 +179,17 @@ __global__ void __launch_bounds__(kThreads) pair_consistency_partial_kernel(
   const unsigned char* mk = mask + pair * hw;
   for (long i = (long)blockIdx.x * kThreads + threadIdx.x; i < hw; i += P * kThreads) {
     if (mk[i] != 0) continue;
-    const float2 f = *reinterpret_cast<const float2*>(fl + 2 * i);
-    const double x = (double)(i % W), y = (double)(i / W);
-    const double qx = __dadd_rn(x, (double)f.x), qy = __dadd_rn(y, (double)f.y);
-    if (!isfinite(qx) || !isfinite(qy)) continue;
-    // border-clamped bilinear taps at q (align_corners=True: pixel centres at integer coordinates)
-    const double ix = fmin(fmax(qx, 0.0), (double)(W - 1)), iy = fmin(fmax(qy, 0.0), (double)(H - 1));
-    const double x0f = floor(ix), y0f = floor(iy);
-    const int x0 = (int)x0f, y0 = (int)y0f, x1 = min(x0 + 1, W - 1), y1 = min(y0 + 1, H - 1);
-    const double wx1 = __dsub_rn(ix, x0f), wy1 = __dsub_rn(iy, y0f);
-    const double wx0 = __dsub_rn(1.0, wx1), wy0 = __dsub_rn(1.0, wy1);
+    FlowTaps t;
+    if (!flow_taps(i, H, W, *reinterpret_cast<const float2*>(fl + 2 * i), t)) continue;
     const bool stat = motion_seg != nullptr && motion_seg[fa * hw + i] == 0;
 #pragma unroll
     for (int src = 0; src < 2; ++src) {
       const float* D = src == 0 ? depth : depth_nn;
-      const float daf = D[fa * hw + i];
-      if (!valid_depth(daf)) continue;
-      const float* Db = D + fb * hw;
-      const float t00 = Db[(long)y0 * W + x0], t01 = Db[(long)y0 * W + x1], t10 = Db[(long)y1 * W + x0],
-                  t11 = Db[(long)y1 * W + x1];
-      if (!valid_depth(t00) || !valid_depth(t01) || !valid_depth(t10) || !valid_depth(t11)) continue;
-      const double da = (double)daf;
-      const double db = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(__dmul_rn(wy0, wx0), (double)t00),
-                                                      __dmul_rn(__dmul_rn(wy0, wx1), (double)t01)),
-                                            __dmul_rn(__dmul_rn(wy1, wx0), (double)t10)),
-                                  __dmul_rn(__dmul_rn(wy1, wx1), (double)t11));
-      // P = R_a (d_a Kinv_a (x, y, 1)) + t_a;  c = R_b^T (P - t_b)
-      double cv[3], pw[3], c[3];
-#pragma unroll
-      for (int r = 0; r < 3; ++r) cv[r] = __dmul_rn(da, dot3(A[9 + r], A[12 + r], A[15 + r], x, y, 1.0));
-#pragma unroll
-      for (int r = 0; r < 3; ++r) pw[r] = __dsub_rn(__dadd_rn(dot3(A[18 + 3 * r], A[19 + 3 * r], A[20 + 3 * r], cv[0], cv[1], cv[2]),
-                                                              A[27 + r]),
-                                                    B[27 + r]);
-#pragma unroll
-      for (int r = 0; r < 3; ++r) c[r] = dot3(B[18 + r], B[21 + r], B[24 + r], pw[0], pw[1], pw[2]);
-      const double z = c[2];
-      double* a = acc + 12 * src;
-      if (!(z > 1e-3)) {
-        a[1] = __dadd_rn(a[1], 1.0);
-        if (stat) a[7] = __dadd_rn(a[7], 1.0);
-        continue;
-      }
-      const double px = __ddiv_rn(dot3(B[0], B[3], B[6], c[0], c[1], c[2]), z);
-      const double py = __ddiv_rn(dot3(B[1], B[4], B[7], c[0], c[1], c[2]), z);
-      const double ex = __dsub_rn(px, qx), ey = __dsub_rn(py, qy);
-      const double er = __dsqrt_rn(__dadd_rn(__dmul_rn(ex, ex), __dmul_rn(ey, ey)));
-      const double ed = __ddiv_rn(fabs(__dsub_rn(z, db)), db);
-#pragma unroll
-      for (int reg = 0; reg < 2; ++reg) {
-        if (reg == 1 && !stat) break;
-        double* s = a + 6 * reg;
-        s[0] = __dadd_rn(s[0], 1.0);
-        s[2] = __dadd_rn(s[2], er);
-        s[3] = __dadd_rn(s[3], ed);
-        s[4] = __dadd_rn(s[4], er < 1.0 ? 1.0 : 0.0);
-        s[5] = __dadd_rn(s[5], er < 3.0 ? 1.0 : 0.0);
-      }
+      double er = 0.0, ed = 0.0;
+      const int res = pair_pixel<false>(cm[0], cm[1], D + fa * hw, D + fb * hw, i, t, nullptr, hw, er, ed);
+      if (res == kNotEvaluated) continue;
+      add_pixel(acc + 12 * src, res, er, ed);
+      if (stat) add_pixel(acc + 12 * src + 6, res, er, ed);
     }
   }
   block_sums<kPairSlots>(acc, red, partials + (pair * P + blockIdx.x) * kPairSlots);

@@ -163,22 +163,25 @@ def pair_consistency(depth, depth_nn, cam, ia, ib, flows, masks, motion_seg=None
     """Device resident frames depth, depth_nn [F,H,W], cam [F,30] and optional motion_seg [F,H,W] uint8; pairs ia, ib (frame
     indices) with host flows [P,H,W,2] fp32 and masks [P,H,W] uint8 (sequences of arrays or tensors). The flows go to the device
     `chunk` pairs per copy. Returns host sums [P,2,2,6] (dvd_pair_consistency's layout)."""
-    F, H, W = depth.shape
-    HW, P = H * W, len(ia)
+    P = len(ia)
     out = []
     for s in range(0, P, int(chunk)):
-        e = min(s + int(chunk), P)
-        n = e - s
-        buf = np.empty(n * HW * 9 + 8 * n, dtype=np.uint8)     # flows, then ia, ib, then masks: the chunk's one copy
-        buf[:n * HW * 8].view(F32).reshape(n, H, W, 2)[:] = np.stack([np.asarray(flows[i], F32) for i in range(s, e)])
-        buf[n * HW * 8:n * HW * 8 + 8 * n].view(np.int32)[:] = np.concatenate([np.asarray(ia[s:e]), np.asarray(ib[s:e])])
-        buf[n * HW * 8 + 8 * n:].reshape(n, H, W)[:] = np.stack([np.asarray(masks[i], np.uint8) for i in range(s, e)])
-        g = torch.from_numpy(buf).to(depth.device)
-        fl = g[:n * HW * 8].view(torch.float32).view(n, H, W, 2)
-        idx = g[n * HW * 8:n * HW * 8 + 8 * n].view(torch.int32)
-        mk = g[n * HW * 8 + 8 * n:].view(n, H, W)
-        out.append(ops.pair_consistency(depth, depth_nn, cam, idx[:n], idx[n:], fl, mk, motion_seg))
+        fl, ia_d, ib_d, mk = upload_pairs(depth.device, depth.shape[1:], ia, ib, flows, masks, s, min(s + int(chunk), P))
+        out.append(ops.pair_consistency(depth, depth_nn, cam, ia_d, ib_d, fl, mk, motion_seg))
     return torch.cat(out).cpu().numpy()
+
+
+def upload_pairs(device, hw, ia, ib, flows, masks, s, e):
+    """pairs s..e-1 in one host-to-device copy: (flow [n,H,W,2] fp32, ia, ib [n] int32, mask [n,H,W] uint8) device views"""
+    H, W = hw
+    HW, n = H * W, e - s
+    buf = np.empty(n * HW * 9 + 8 * n, dtype=np.uint8)         # flows, then ia, ib, then masks
+    buf[:n * HW * 8].view(F32).reshape(n, H, W, 2)[:] = np.stack([np.asarray(flows[i], F32) for i in range(s, e)])
+    buf[n * HW * 8:n * HW * 8 + 8 * n].view(np.int32)[:] = np.concatenate([np.asarray(ia[s:e]), np.asarray(ib[s:e])])
+    buf[n * HW * 8 + 8 * n:].reshape(n, H, W)[:] = np.stack([np.asarray(masks[i], np.uint8) for i in range(s, e)])
+    g = torch.from_numpy(buf).to(device)
+    idx = g[n * HW * 8:n * HW * 8 + 8 * n].view(torch.int32)
+    return g[:n * HW * 8].view(torch.float32).view(n, H, W, 2), idx[:n], idx[n:], g[n * HW * 8 + 8 * n:].view(n, H, W)
 
 
 # ---- the whole export ---------------------------------------------------------------------------------------------------------

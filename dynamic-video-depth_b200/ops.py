@@ -1268,3 +1268,91 @@ def pair_consistency(depth, depth_nn, cam, ia, ib, flow, mask, motion_seg=None):
     _lib.check(lib.dvd_pair_consistency(_ptr(depth), _ptr(depth_nn), _ptr(cam), F, _ptr(ia), _ptr(ib), _ptr(flow), _ptr(mask),
                                         _ptr(motion_seg), _ptr(sums), _ptr(partials), P, H, W, _stream()), 'dvd_pair_consistency')
     return sums
+
+
+# ---- the learned scene flow over a test export (csrc/tracks.cu) ---------------------------------------------------------------
+SF_REGIONS = 3               # all, static, moving
+
+
+def pair_consistency_sf(depth, cam, ia, ib, flow, mask, sf, motion_seg=None):
+    """dvd_pair_consistency_sf: resident frames depth [F,H,W] fp32 (the refined depth) and cam [F,30] fp32 (points.camera_block),
+    pairs ia, ib [P] int32, flow [P,H,W,2] fp32, mask [P,H,W] uint8 (flowpair mask_2), sf [P,3,H,W] fp32 (each pair's scene flow
+    on frame a's grid), motion_seg [F,H,W] uint8 or None -> sums [P,3,6] fp64 per region (all, static, moving): pair_consistency's
+    sums with sf added to the world point."""
+    _chk(depth, 'depth')
+    if depth.dim() != 3:
+        raise ValueError('depth must be [F,H,W], got %s' % (tuple(depth.shape),))
+    F, H, W = depth.shape
+    _chk(cam, 'cam', (F, 30))
+    _chk_dtype(ia, 'ia', torch.int32, 1)
+    P = ia.shape[0]
+    _chk_dtype(ib, 'ib', torch.int32, 1)
+    _chk(flow, 'flow', (P, H, W, 2))
+    _chk(sf, 'sf', (P, 3, H, W))
+    _chk_dtype(mask, 'mask', torch.uint8, 3)
+    if tuple(ib.shape) != (P,) or tuple(mask.shape) != (P, H, W):
+        raise ValueError('ib must be [%d] and mask [%d,%d,%d], got %s and %s' % (P, P, H, W, tuple(ib.shape), tuple(mask.shape)))
+    if motion_seg is not None:
+        _chk_dtype(motion_seg, 'motion_seg', torch.uint8, 3)
+        if tuple(motion_seg.shape) != (F, H, W):
+            raise ValueError('motion_seg must be [%d,%d,%d], got %s' % (F, H, W, tuple(motion_seg.shape)))
+    _same_device('pair_consistency_sf', depth, cam, ia, ib, flow, mask, sf, motion_seg)
+    if not 1 <= P <= 65535:
+        raise ValueError('pair_consistency_sf takes 1 to 65535 pairs per call, got %d' % P)
+    if int(ia.min()) < 0 or int(ib.min()) < 0 or int(ia.max()) >= F or int(ib.max()) >= F:
+        raise ValueError('pair frame indices must lie in [0, %d)' % F)
+    lib = _lib.load()
+    partials = torch.empty(lib.dvd_pair_consistency_sf_partials_size(P, H, W), dtype=torch.float64, device=depth.device)
+    sums = torch.empty(P, SF_REGIONS, PAIR_SLOTS, dtype=torch.float64, device=depth.device)
+    LAUNCHES['n'] += 2
+    _lib.check(lib.dvd_pair_consistency_sf(_ptr(depth), _ptr(cam), F, _ptr(ia), _ptr(ib), _ptr(flow), _ptr(mask), _ptr(motion_seg),
+                                           _ptr(sf), _ptr(sums), _ptr(partials), P, H, W, _stream()), 'dvd_pair_consistency_sf')
+    return sums
+
+
+def draw_tracks(X, first, length, rgb, cams, depth, img, number, tail, proj=None, vis=None):
+    """dvd_draw_tracks: tracks X [M,L1,3] fp32 (world positions; position k of track i belongs to frame number first[i] + k),
+    first, length [M] int32 (alive positions, 1..L1), rgb [M,3] uint8, drawn over the frames cams [F,21] fp32
+    (render_views.view_cams), depth [F,H,W] fp32, img [F,3,H,W] fp32, number [F] int32 (frame numbers) with the exact rule of
+    include/dvd_b200.h -> out [F,H,W,3] uint8 BGR. proj [M,L1,3] fp32 and vis [M,L1] uint8, when given,
+    receive the head projection and visibility of every (track, position) drawn in these frames; other entries keep their
+    values."""
+    _chk(depth, 'depth')
+    if depth.dim() != 3:
+        raise ValueError('depth must be [F,H,W], got %s' % (tuple(depth.shape),))
+    F, H, W = depth.shape
+    _chk(X, 'X')
+    if X.dim() != 3 or X.shape[2] != 3 or X.shape[1] < 1:
+        raise ValueError('X must be [M,L1,3] with L1 >= 1, got %s' % (tuple(X.shape),))
+    M, L1 = X.shape[0], X.shape[1]
+    _chk_dtype(first, 'first', torch.int32, 1)
+    _chk_dtype(length, 'length', torch.int32, 1)
+    _chk_dtype(rgb, 'rgb', torch.uint8, 2)
+    _chk_dtype(number, 'number', torch.int32, 1)
+    if first.shape[0] != M or length.shape[0] != M or tuple(rgb.shape) != (M, 3) or number.shape[0] != F:
+        raise ValueError('first, length must be [%d], rgb [%d,3] and number [%d]' % (M, M, F))
+    _chk(cams, 'cams', (F, _lib.DVD_VIEW_CAM_FLOATS))
+    _chk(img, 'img', (F, 3, H, W))
+    if not 0 <= int(tail) <= _lib.DVD_TRACK_MAX_TAIL or int(tail) != tail:
+        raise ValueError('tail must be an integer in [0, %d], got %r' % (_lib.DVD_TRACK_MAX_TAIL, tail))
+    if not 1 <= F <= 65535:
+        raise ValueError('draw_tracks takes 1 to 65535 frames per call, got %d' % F)
+    if M >= 2 ** 31:
+        raise ValueError('draw_tracks takes fewer than 2^31 tracks, got %d' % M)
+    if (proj is None) != (vis is None):
+        raise ValueError('give both proj and vis, or neither')
+    if proj is not None:
+        _chk(proj, 'proj', (M, L1, 3))
+        _chk_dtype(vis, 'vis', torch.uint8, 2)
+        if tuple(vis.shape) != (M, L1):
+            raise ValueError('vis must be [%d,%d], got %s' % (M, L1, tuple(vis.shape)))
+    _same_device('draw_tracks', X, first, length, rgb, cams, depth, img, number, proj, vis)
+    if M and (int(length.min()) < 1 or int(length.max()) > L1):
+        raise ValueError('length must lie in [1, %d]' % L1)
+    keys = torch.empty(F, H, W, dtype=torch.int64, device=depth.device)
+    out = torch.empty(F, H, W, 3, dtype=torch.uint8, device=depth.device)
+    LAUNCHES['n'] += 3 if M else 2
+    _lib.check(_lib.load().dvd_draw_tracks(_ptr(X), _ptr(first), _ptr(length), _ptr(rgb), M, L1, _ptr(cams), _ptr(depth), _ptr(img),
+                                           _ptr(number), F, H, W, int(tail), _ptr(keys), _ptr(out), _ptr(proj), _ptr(vis), _stream()),
+               'dvd_draw_tracks')
+    return out

@@ -522,6 +522,46 @@ int dvd_pair_consistency(const float* depth, const float* depth_nn, const float*
                          const float* flow, const unsigned char* mask, const unsigned char* motion_seg, double* sums,
                          double* partials, int n_pairs, int H, int W, void* stream);
 
+/* ---- the learned scene flow over a test export (csrc/tracks.cu, dvd_b200.tracks). ------------------------------------------
+ * dvd_pair_consistency_sf: dvd_pair_consistency for one depth source, `depth`, with the scene flow sf [n_pairs,3,H,W] fp32 of
+ * each pair (channel-planar, the pair's frame a grid) added to the world point: P' = P + (double)sf(x) component by component,
+ * after P = R_a (D_a(x) Kinv_a (i, j, 1)) + t_a is formed, and c = R_b^T (P' - t_b). Everything else (the evaluated-pixel
+ * rule, D~, behind, e_r, e_d, the sums and their order) is dvd_pair_consistency's, through the same device code, so sf = 0
+ * gives its `depth` sums bit for bit. sums [n_pairs,3,6] fp64 per region: 0 all, 1 static (motion_seg of frame a is 0), 2
+ * moving (motion_seg of frame a is not 0); regions 1 and 2 are zero without motion_seg. partials: fp64 words.               */
+long long dvd_pair_consistency_sf_partials_size(int n_pairs, int H, int W);
+int dvd_pair_consistency_sf(const float* depth, const float* cam, int n_frames, const int* ia, const int* ib, const float* flow,
+                            const unsigned char* mask, const unsigned char* motion_seg, const float* sf, double* sums,
+                            double* partials, int n_pairs, int H, int W, void* stream);
+/* dvd_draw_tracks: 3D tracks drawn over F frames. Track i (< M < 2^31) starts at frame number first[i] and has len[i] <= L1
+ * positions X[i, 0..len-1] (X [M,L1,3] fp32, world space): position k belongs to frame number first[i] + k. Frame f (number[f],
+ * int32) has the view block cams[f] ([F,21] fp32: w2c 3x4 | K 3x3, row-major, as dvd_splat_views), its refined depth
+ * [F,H,W] fp32 and its image img [F,3,H,W] fp32 RGB. In frame f a track with k = number[f] - first[i] in [0, len[i]) is drawn:
+ *   projection (render_views'): q = w2c X (each row ((w0 x + w1 y) + w2 z) + w3), h = K q (((k0 q0 + k1 q1) + k2 q2)),
+ *     u = h0 / h2, v = h1 / h2, all fp32 with every operation rounded on its own; dropped when q2 <= 1e-2f or q0, q1, q2, u or
+ *     v is not finite; z = q2; its pixel is (floor(u + 0.5f), floor(v + 0.5f)).
+ *   a sample (pixel, z) is plotted when the pixel is in the image and not hidden: hidden when the frame's depth d there is valid
+ *     (finite, > 1e-2f) and z > d * DVD_TRACK_HIDE_TOL (fp32 product).
+ *   head, rank 0: the (2 DVD_TRACK_HEAD_RADIUS + 1)^2 pixels around X[i,k]'s pixel, each with X[i,k]'s z.
+ *   segments X[i,j] -> X[i,j+1] for j = max(0, k - tail) .. k - 1, rank k - j, when both ends project: du = u1 - u0, dv, dz
+ *     likewise, S = max(1, min(DVD_TRACK_MAX_SAMPLES, ceil(max(|du|, |dv|)))), samples s = 0..S at t = s / S: (u0 + t du,
+ *     v0 + t dv, z0 + t dz).
+ *   each plotted sample min-accumulates the key (rank << 32) | i into its pixel (atomicMin): youngest rank first, then the lower
+ *     track index, whatever the order.
+ *   resolve: base = (uint8)(255 clip(img, 0, 1)) with NaN -> 0; a pixel with a key takes w = 256 (tail + 1 - rank) / (tail + 1)
+ *     (integer division) and (c w + base (256 - w) + 128) >> 8 per channel, c = rgb[i] (uint8 RGB [M,3]). out [F,H,W,3] uint8
+ *     BGR. keys [F,H,W] uint64 is the work buffer (filled here).
+ * proj [M,L1,3] fp32 and vis [M,L1] uint8 may both be NULL; else, for every drawn (i, k), proj[i,k] = (u, v, z) of the head (NaN
+ * when dropped) and vis[i,k] = 1 when its centre sample is plotted, else 0. Other entries are left as they are. 0 <= tail <=
+ * DVD_TRACK_MAX_TAIL, 1 <= F <= 65535.                                                                                      */
+#define DVD_TRACK_HIDE_TOL 1.05f
+#define DVD_TRACK_HEAD_RADIUS 1
+#define DVD_TRACK_MAX_SAMPLES 1024
+#define DVD_TRACK_MAX_TAIL 64
+int dvd_draw_tracks(const float* X, const int* first, const int* len, const unsigned char* rgb, int M, int L1, const float* cams,
+                    const float* depth, const float* img, const int* number, int F, int H, int W, int tail,
+                    unsigned long long* keys, unsigned char* out, float* proj, unsigned char* vis, void* stream);
+
 /* ---- test-end visualisation (csrc/test_videos.cu): models/video_base.py:157-272 (on_test_end) without matplotlib. ----------- */
 #define DVD_VIS_MAX_PANELS 4
 enum { DVD_VIS_DISP = 0, DVD_VIS_GT_DISP = 1, DVD_VIS_RGB = 2 };
